@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — BASELINE.json metric: "edges/sec in F-gradient step at 1/2/4/8 B200; iters/sec on
+"""bench.py — BASELINE.json metric: "edges/sec in F-gradient step at 1/2/4/8 H100; iters/sec on
 com-amazon K=200".
 
 A step = one call of the hot path (backtrackingLineSearchs, codes/bigclam4-7.scala:152-223: PRE +
@@ -35,11 +35,13 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
 import numpy as np
 
+sys.dont_write_bytecode = True          # the tree may be read-only: nothing is cached there
 REPO = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, REPO)
 
@@ -108,7 +110,7 @@ def hbm_peak():
     p = os.path.join(REPO, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -178,7 +180,7 @@ def load_oracle_all_cores():
     os.environ["OMP_NUM_THREADS"] = str(host_cores())
     os.environ.pop("OMP_THREAD_LIMIT", None)
     from oracle import oracle as O
-    O.build()
+    O.build(out_dir=tempfile.mkdtemp(prefix="bigclam_oracle_"))      # a rebuild, if one is needed, stays out of the tree
     return O
 
 
@@ -281,6 +283,30 @@ def sparse_layout_bytes(indptr, rp, col):
     return int(blk[col].sum() + 12 * len(col) + 2 * blk.sum() + 16 * (len(rp) - 1))
 
 
+DUMP_BYTES = 48 << 20       # F is n x K doubles (535 MB at com-amazon K=200): a fixed sample of its rows is written
+
+
+def dump_outputs(out_dir, b, sparse):
+    """What the timed path hands its caller after the last timed step: F (a fixed, seeded sample of its rows when the
+    whole matrix is larger than DUMP_BYTES), sumF and the LLH of every timed step, as float64 .npy files."""
+    n, k = b.n, b.K
+    m = min(n, DUMP_BYTES // (8 * k))
+    rows = np.arange(n) if m == n else np.sort(np.random.default_rng(2024).choice(n, size=m, replace=False))
+    if sparse:
+        indptr, indices, values = b.F_csr()
+        F = np.zeros((m, k))
+        cnt = np.diff(indptr)[rows]
+        src = np.repeat(indptr[rows] - np.concatenate(([0], np.cumsum(cnt)[:-1])), cnt) + np.arange(cnt.sum())
+        F[np.repeat(np.arange(m), cnt), indices[src]] = values[src]
+    else:
+        F = b.F[rows]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "F_rows.npy"), F)
+    np.save(os.path.join(out_dir, "F_row_ids.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "sumF.npy"), b.sumF)
+    np.save(os.path.join(out_dir, "llh_trace.npy"), np.asarray(b.last_trace, dtype=np.float64))
+
+
 class ExtrasWatchdog:
     """The headline numbers (value, roofline, e2e) are measured first; everything after them (the reference-style-init
     workload, the exhaustive-line-search arm, the run to convergence, the ncu side process, the CPU baseline) explains them.
@@ -354,6 +380,8 @@ def run_single(args):
     torch.cuda.synchronize()
     clocks = sampler.stop()
     assert b.last_calls == args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, b, sparse)
     total_ms = e0.elapsed_time(e1)
     kern_ms, n_step_kernels, n_all = b.kernel_time()
     ms_per_step = total_ms / args.steps
@@ -537,7 +565,13 @@ def main():
     ap.add_argument("--no-line-search", action="store_true", help="skip the exhaustive-line-search arm and the run to convergence")
     ap.add_argument("--extras-limit", type=float, default=420.0,
                     help="seconds the explanatory legs after the timed regions may take before the line is printed without them")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write F (seeded row sample), sumF and the LLH trace of the timed path as DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "b200" or args.gpus > 1 or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs is implemented for the single-GPU arm")
     cfg = CONFIGS[args.config]
     args.graph = args.graph or cfg["graph"]
     args.k = args.k or cfg["k"]

@@ -1,4 +1,4 @@
-"""bigclam_apachespark_b200 — B200-native drop-in for the F-gradient / line-search step of
+"""bigclam_apachespark_b200 — H100-native drop-in for the F-gradient / line-search step of
 thangdnsf/BigCLAM-ApacheSpark (`backtrackingLineSearchs`, codes/bigclam4-7.scala:152-223).
 
 Only what the hot path needs lives here: the CUDA kernels + C ABI (csrc/, libbigclam_b200.so)

@@ -1,4 +1,4 @@
-// bigclam_capi.cu — C ABI (include/bigclam_b200.h) over the sm_100a kernels.
+// bigclam_capi.cu — C ABI (include/bigclam_b200.h) over the sm_90a kernels.
 // No CPU fallback: every compute entry point launches CUDA kernels or fails.
 #include "../../include/bigclam_b200.h"
 #include "bigclam_kernels.cuh"
@@ -162,7 +162,7 @@ static int drop_speculation(bigclam_ctx *ctx) {
 static int ensure_dense(bigclam_ctx *ctx);
 static int check_overflow(bigclam_ctx *ctx);
 
-extern "C" const char *bigclam_version(void) { return "bigclam_b200 0.1 (sm_100a)"; }
+extern "C" const char *bigclam_version(void) { return "bigclam_b200 0.1 (sm_90a)"; }
 
 extern "C" int bigclam_device_count(void) {
     int n = 0;
@@ -522,8 +522,8 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
     cudaDeviceProp prop;
     CUC(cudaGetDeviceProperties(&prop, dev));
     ctx->num_sms = prop.multiProcessorCount;
-    if (prop.major < 10) {
-        fail(nullptr, BIGCLAM_ECUDA, "bigclam_create: device sm_%d%d, this library is built for sm_100a only", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {       // sm_90a code runs on compute capability 9.0 and nothing else
+        fail(nullptr, BIGCLAM_ECUDA, "bigclam_create: device sm_%d%d, this library is built for sm_90a only", prop.major, prop.minor);
         free_ctx(ctx);
         return BIGCLAM_ECUDA;
     }

@@ -1,4 +1,4 @@
-// bigclam_kernels.cuh — sm_100a kernels of the BigCLAM hot path (one warp per node).
+// bigclam_kernels.cuh — sm_90a kernels of the BigCLAM hot path (one warp per node).
 //
 // What one launch of step_kernel computes, per node u (reference: codes/bigclam4-7.scala):
 //   PRE   :157-169  x_uv = fu.fv, p = clamp(exp(-x)), grad_u = sum_v fv/(1-p) - sumF + fu,

@@ -2,8 +2,8 @@
 // deterministic reduction that follows every launch.
 //
 // Why tiles: com-amazon has a mean degree of 5.5 and rows of ~10 non-zeros — a warp that owns ONE such node
-// spends most of its issue slots with 5 of 32 lanes busy (the one-warp-per-node kernels execute 2,900 warp
-// instructions per node, see profiles/r2_sparse_warp_per_node_ncu.txt).  A tile is a run of up to 8 consecutive
+// spends most of its issue slots with 5 of 32 lanes busy (the one-warp-per-node kernels execute ~2,900 warp
+// instructions per node).  A tile is a run of up to 8 consecutive
 // nodes of the degree-sorted processing order with at most 32 edges in total, handled by one warp; every phase
 // maps its work items flat onto the 32 lanes:
 //   stage   one bulk copy (cp.async.bulk.shared::cluster.global + mbarrier) per neighbour row and per own row;

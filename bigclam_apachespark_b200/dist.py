@@ -2,7 +2,7 @@
 
 The reference's only parallelism is Spark data-parallel `map` over nodes with the whole F matrix
 broadcast to every executor each call (codes/bigclam4-7.scala:154) and driver-side reduces
-(:191-192, :219).  The B200 equivalent (DESIGN.md (e)):
+(:191-192, :219).  The H100 equivalent (DESIGN.md (e)):
 
   * every rank keeps the CSR and a replica of F (n x ld fp64, double-buffered) in its own HBM;
     rank r owns the contiguous node range [bounds[r], bounds[r+1]) (balanced by neighbour-list

@@ -1,5 +1,5 @@
 /*
- * bigclam_b200.h — C ABI of the B200-native BigCLAM F-gradient / line-search step.
+ * bigclam_b200.h — C ABI of the H100-native BigCLAM F-gradient / line-search step.
  *
  * The reference (thangdnsf/BigCLAM-ApacheSpark) has no FFI or plugin interface; its boundary is
  * the implicit signature of one spark-shell function and the globals it touches:

@@ -52,22 +52,27 @@ def _cpu_tag() -> str:
     return "unknown"
 
 
-def build(force: bool = False) -> str:
+def build(force: bool = False, out_dir: str | None = None) -> str:
     """Compile liboracle.so from the C restatement (gcc + OpenMP, -O3 -march=native); returns its path.  The
-    library is rebuilt when the source is newer or when it was built for another CPU model (it travels with the
-    repository snapshot to the GPU box, whose host CPU may differ)."""
+    library is rebuilt when the source is newer or when it was built for another CPU model (a copied tree may
+    land on a host whose CPU differs).  out_dir: where a rebuild goes instead of oracle/ (callers that must not
+    write into the tree); the library found current is used from wherever it is."""
+    global _LIB_PATH
     src = os.path.join(_HERE, "bigclam_oracle.c")
-    tag_path = os.path.join(_HERE, "liboracle.host")
     tag = _cpu_tag()
     try:
-        with open(tag_path) as fh:
+        with open(os.path.join(os.path.dirname(_LIB_PATH), "liboracle.host")) as fh:
             same_cpu = fh.read().strip() == tag
     except OSError:
         same_cpu = False
     if force or not same_cpu or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < os.path.getmtime(src):
-        subprocess.run(["make", "-C", _HERE, "-B"], check=True, stdout=subprocess.DEVNULL)
-        with open(tag_path, "w") as fh:
+        d = out_dir or _HERE
+        os.makedirs(d, exist_ok=True)
+        out = os.path.join(d, "liboracle.so")
+        subprocess.run(["make", "-C", _HERE, "-B", f"OUT={out}"], check=True, stdout=subprocess.DEVNULL)
+        with open(os.path.join(d, "liboracle.host"), "w") as fh:
             fh.write(tag + "\n")
+        _LIB_PATH = out
     return _LIB_PATH
 
 
@@ -77,8 +82,7 @@ _lib = None
 def lib() -> C.CDLL:
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(_LIB_PATH)
+        L = C.CDLL(build())
         dp = C.POINTER(C.c_double)
         L.oracle_step_sizes.argtypes = [C.c_double, C.c_int32, dp]
         L.oracle_step_sizes.restype = None

@@ -204,7 +204,7 @@ typedef void *cudaStream_t;
 struct emu_event { std::chrono::steady_clock::time_point t; };
 typedef emu_event *cudaEvent_t;
 struct cudaIpcMemHandle_t { char reserved[64]; };
-struct cudaDeviceProp { int major = 10, minor = 0, multiProcessorCount = 1; };
+struct cudaDeviceProp { int major = 9, minor = 0, multiProcessorCount = 1; };
 enum cudaMemcpyKind { cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice, cudaMemcpyHostToHost };
 enum { cudaStreamNonBlocking = 1, cudaIpcMemLazyEnablePeerAccess = 1, cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
 inline const char *cudaGetErrorString(cudaError_t) { return "emulated runtime error"; }

@@ -9,7 +9,7 @@ tests build such a caller with the C compiler of the image and
   and that its own logic — reader, F0 file, bigclam_run / bigclam_multi_run, getters, output file — is right by
   running it against the host-emulation build of the same C API (tests/emu/build_hostemu.sh) and the oracle;
 * (`-m gpu`, tests/test_gpu_zy_c_host.py — collected next to last so that a problem here cannot hide the parity
-  results of the suite under `-x`) run it on the B200 against the product library: edge list -> SGDFindC to the reference's stop rule ->
+  results of the suite under `-x`) run it on the H100 against the product library: edge list -> SGDFindC to the reference's stop rule ->
   F, sumF, LLH trace, compared with the oracle's outer loop (bigclam4-7.scala:225-243) from the same F0; and the
   `init` mode (GPU ego-net conductance + initNeighborComF, :58-108) against the driver's own path.
 """
@@ -145,7 +145,7 @@ def test_c_caller_fails_loudly_without_a_device(tmp_path):
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("world", [1, 2])
 def test_c_caller_logic_under_host_emulation(oracle, tmp_path, world):
-    """The program itself (not the kernels' sm_100a code) against the oracle: linked with the host-emulation build of the
+    """The program itself (not the kernels' sm_90a code) against the oracle: linked with the host-emulation build of the
     C API, which runs the same sources on OS threads.  Test infrastructure only."""
     emu = os.path.join(EMU_DIR, "libbigclam_hostemu.so")
     if not os.path.exists(emu):

@@ -1,7 +1,7 @@
 """Kernel LOGIC on the CPU: the source of the DENSE kernels (csrc/bigclam_kernels.cuh) compiled for the host against the SIMT
 emulation in tests/emu (one OS thread per CUDA thread, warp collectives as barrier rounds) and checked against
 the oracle.  Test infrastructure only — nothing here is reachable from the package, which has no CPU path; the
-`-m gpu` tests remain the parity tests of the compiled sm_100a code.  (The sparse-row engine runs under the same
+`-m gpu` tests remain the parity tests of the compiled sm_90a code.  (The sparse-row engine runs under the same
 emulation through the host build of the whole C API: tests/test_hostemu_sparse.py.)"""
 import ctypes as C
 import os

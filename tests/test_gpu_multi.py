@@ -1,7 +1,6 @@
 """All the GPUs of one box through the C ABI only (bigclam_multi_*: no torch.distributed, no NCCL): one context per
 device, fused NVLink row pushes and the fused collective, against the oracle and against the single-GPU path.
-Needs >= 2 GPUs (skipped on the 1-GPU test box; `gpurun --gpus 2/4/8 -- python -m pytest tests/test_gpu_multi.py -m gpu`
-logs are kept under profiles/).  Under the host-emulation build (BIGCLAM_HOSTEMU=1) the "devices" are emulated and the
+Needs >= 2 GPUs (skipped on a 1-GPU machine: `python -m pytest tests/test_gpu_multi.py -m gpu` on a box with 2/4/8).  Under the host-emulation build (BIGCLAM_HOSTEMU=1) the "devices" are emulated and the
 test runs on the CPU (tests/test_hostemu_sparse.py drives it)."""
 import os
 

@@ -1,4 +1,4 @@
-"""`-m gpu` part of tests/test_c_host.py: the plain-C caller (tests/c_host/sgd_find_c.c) on the B200 against the product
+"""`-m gpu` part of tests/test_c_host.py: the plain-C caller (tests/c_host/sgd_find_c.c) on the H100 against the product
 library — edge list -> SGDFindC to the reference's stop rule (bigclam4-7.scala:225-243) -> F, sumF, LLH trace against the
 oracle's outer loop from the same F0; two GPUs behind one handle; the `init` mode against the Python driver."""
 import os

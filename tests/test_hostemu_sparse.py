@@ -4,8 +4,8 @@ tests/test_gpu_sparse.py is run, in a child pytest, against the HOST-EMULATION b
 emulation of tests/emu/include/cuda_emu.h — one OS thread per CUDA thread, warp collectives as barrier rounds, so a
 collective reached by part of a warp hangs instead of passing).  The tile path, the general path, split hubs, the
 fixed-order reduction, the pool / CSR entry points and the device-side loop bookkeeping all run here against the
-oracle.  Test infrastructure only: the product library has no CPU path and the `-m gpu` tests on the B200 remain
-the parity tests of the compiled sm_100a code."""
+oracle.  Test infrastructure only: the product library has no CPU path and the `-m gpu` tests on the H100 remain
+the parity tests of the compiled sm_90a code."""
 import os
 import subprocess
 import sys

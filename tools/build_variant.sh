@@ -11,7 +11,7 @@ cp bigclam_apachespark_b200/csrc/bigclam_capi.cu bigclam_apachespark_b200/csrc/i
 # kernel header: tools/ab/<name>.cuh when it exists, else the product one (variants made of -D flags only)
 if test -f tools/ab/$name.cuh; then cp tools/ab/$name.cuh $tmp/pkg/csrc/bigclam_kernels.cuh; else cp bigclam_apachespark_b200/csrc/bigclam_kernels.cuh $tmp/pkg/csrc/; fi
 cp bigclam_apachespark_b200/csrc/bigclam_sparse.cuh bigclam_apachespark_b200/csrc/bigclam_tile.cuh $tmp/pkg/csrc/
-/usr/local/cuda/bin/nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -ccbin /usr/bin/g++ \
+/usr/local/cuda/bin/nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -ccbin /usr/bin/g++ \
     -Xcompiler -fPIC,-O3 -Xptxas -v --expt-relaxed-constexpr "$@" -shared -o tools/ab/lib_$name.so \
     $tmp/pkg/csrc/bigclam_capi.cu $tmp/pkg/csrc/initf_gpu.cu $tmp/pkg/csrc/edgelist.cpp $tmp/pkg/csrc/initf.cpp 2> tools/ab/build_$name.log
 grep -A3 "step_kernelILi4ELi[24]ELb0ELb0\|tile_step_kernelILb0ELb0" tools/ab/build_$name.log | grep -E "Used|spill" | head -8

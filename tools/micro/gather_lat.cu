@@ -50,7 +50,7 @@ int main(int argc, char **argv) {
     const int work = argc > 1 ? atoi(argv[1]) : 2000;
     const int dense = argc > 2 ? atoi(argv[2]) : 1;
     double *F; CK(cudaMalloc(&F, sizeof(double) * (size_t)n * ld)); { std::vector<double> hf((size_t)n * ld); unsigned long long st = 88172645463325252ULL; for (auto &v : hf) { st ^= st << 13; st ^= st >> 7; st ^= st << 17; v = ((st >> 11) * (1.0 / 9007199254740992.0)) * (((st & 31) == 0) ? 1.0 : (dense ? 1.0 : 0.0)); } CK(cudaMemcpy(F, hf.data(), hf.size() * 8, cudaMemcpyHostToDevice)); }
-    const int blocks = 148 * 2, warps = blocks * 8, nb = 200;
+    const int blocks = 132 * 2, warps = blocks * 8, nb = 200;
     std::vector<int> h((size_t)warps * nb * 4);
     srand(1);
     for (auto &v : h) v = (int)(((long long)rand() * 32768 + rand()) % n);
