@@ -502,11 +502,6 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
     ctx->hi = n;
     ctx->nsteps = params->max_inter + 1;
     bigclam_step_sizes(params->beta, params->max_inter, ctx->steps);
-    const int ld2 = ld / 2;
-    const int c2raw = (ld2 + 31) / 32;
-    ctx->c2 = c2raw <= 1 ? 1 : c2raw <= 2 ? 2 : c2raw <= 4 ? 4 : c2raw <= 8 ? 8 : 16;
-    ctx->maxm = std::min<int32_t>(ld, kMaxActiveCap);
-    ctx->smem_bytes = block_smem_bytes(ld, ctx->maxm);
 
 #define CUC(call)                                                                                 \
     do {                                                                                          \
@@ -527,23 +522,6 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
         free_ctx(ctx);
         return BIGCLAM_ECUDA;
     }
-    int bps = 0;
-    cudaError_t ce;
-    switch (ctx->c2) {
-        case 1: ce = configure_kernel<1>(ctx->smem_bytes, &bps); break;
-        case 2: ce = configure_kernel<2>(ctx->smem_bytes, &bps); break;
-        case 4: ce = configure_kernel<4>(ctx->smem_bytes, &bps); break;
-        case 8: ce = configure_kernel<8>(ctx->smem_bytes, &bps); break;
-        default: ce = configure_kernel<16>(ctx->smem_bytes, &bps); break;
-    }
-    if (ce != cudaSuccess || bps <= 0) {
-        fail(nullptr, BIGCLAM_ECUDA, "bigclam_create: kernel configuration failed: %s (smem %zu B)",
-             cudaGetErrorString(ce), ctx->smem_bytes);
-        free_ctx(ctx);
-        return BIGCLAM_ECUDA;
-    }
-    ctx->grid = ctx->num_sms * bps;
-    ctx->h_work_init = 3u * (unsigned int)ctx->grid * kWarpsPerBlock;
     if (params->flags & BIGCLAM_F_SPARSE_ROWS) {
         if (params->min_f != 0.0) {
             fail(nullptr, BIGCLAM_EUNSUPPORTED, "bigclam_create: BIGCLAM_F_SPARSE_ROWS needs min_f == 0");
@@ -580,6 +558,29 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
         if (const char *ev = std::getenv("BIGCLAM_LS_EXHAUSTIVE")) ctx->ls_exhaustive = std::atoi(ev) != 0;
         if (const char *ev = std::getenv("BIGCLAM_LS_PRUNE")) ctx->ls_level = std::max(1, std::min(2, std::atoi(ev)));
         if (const char *ev = std::getenv("BIGCLAM_TILE_EDGES")) ctx->tile_edges = std::max(0, std::min(kTlMaxEdges, std::atoi(ev)));
+    } else {
+        // dense rows (step_kernel): a persistent grid of kWarpsPerBlock-warp blocks, C2 double2 chunks of a row per lane
+        const int c2raw = (ld / 2 + 31) / 32;
+        ctx->c2 = c2raw <= 1 ? 1 : c2raw <= 2 ? 2 : c2raw <= 4 ? 4 : c2raw <= 8 ? 8 : 16;
+        ctx->maxm = std::min<int32_t>(ld, kMaxActiveCap);
+        ctx->smem_bytes = block_smem_bytes(ld, ctx->maxm);
+        int bps = 0;
+        cudaError_t ce;
+        switch (ctx->c2) {
+            case 1: ce = configure_kernel<1>(ctx->smem_bytes, &bps); break;
+            case 2: ce = configure_kernel<2>(ctx->smem_bytes, &bps); break;
+            case 4: ce = configure_kernel<4>(ctx->smem_bytes, &bps); break;
+            case 8: ce = configure_kernel<8>(ctx->smem_bytes, &bps); break;
+            default: ce = configure_kernel<16>(ctx->smem_bytes, &bps); break;
+        }
+        if (ce != cudaSuccess || bps <= 0) {
+            fail(nullptr, BIGCLAM_ECUDA, "bigclam_create: kernel configuration failed: %s (smem %zu B)",
+                 cudaGetErrorString(ce), ctx->smem_bytes);
+            free_ctx(ctx);
+            return BIGCLAM_ECUDA;
+        }
+        ctx->grid = ctx->num_sms * bps;
+        ctx->h_work_init = 3u * (unsigned int)ctx->grid * kWarpsPerBlock;
     }
 
     CUC(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
