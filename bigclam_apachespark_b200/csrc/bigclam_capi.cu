@@ -46,7 +46,7 @@ struct bigclam_ctx {
     double *d_partials = nullptr;
     int8_t *d_accepted = nullptr;   // accepted step index per node of the last COMMITTED step
     int8_t *d_accepted_spec = nullptr;   // written by a speculative step (bigclam_step), swapped in at commit
-    bool spec_valid = false;        // the next step has already been computed speculatively (see bigclam_step)
+    bool spec_valid = false;        // the next step has already been computed speculatively (see group_step)
     bool spec_null_mask = true;
     std::vector<uint8_t> spec_mask;    // the uset the speculative step was computed with (exact comparison)
     uint8_t *d_mask = nullptr;
@@ -1207,148 +1207,184 @@ static int reset_run_state(bigclam_ctx *ctx) {
     return BIGCLAM_OK;
 }
 
-extern "C" int bigclam_loglikelihood(bigclam_ctx *ctx, double *llh_out) {
-    if (ctx == nullptr) return BIGCLAM_EINVAL;
-    if (llh_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "bigclam_loglikelihood: llh_out is NULL");
-    CU(cudaSetDevice(ctx->device));
-    int rc = reset_run_state(ctx);
-    if (rc) return rc;
-    StepArgs a;
-    fill_args(ctx, a, false, nullptr, false);
-    rc = timed_launch(ctx, a, false);
-    if (rc) return rc;
-    CU(cudaMemcpyAsync(ctx->h_pinned, ctx->d_partials + 2 * ctx->ld, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    *llh_out = ctx->h_pinned[0];
+// ------------------------------------------------------------------------------------------------
+// backtrackingLineSearchs, loglikelihood and the outer loop on a group of contexts that hold one F between them: one
+// context (bigclam_step, bigclam_loglikelihood, bigclam_run) or the ranks of a bigclam_multi handle, which step the
+// nodes they own, store their new rows into every replica and add up their sums with the fused collective.  An error
+// is recorded on the rank it happened on (fail / CU), and *bad says which rank that was.  Rank 0's device is made
+// current on entry and is current between passes over the ranks, so one context sets its device once per call.
+
+// f(ctx) on every rank in rank order, with that rank's device current.  Stops at the first error with *bad at that
+// rank; otherwise leaves *bad at 0 and rank 0's device current, so that the caller can go on with CU on rank 0.
+template <class Fn>
+static int each_rank(bigclam_ctx *const *r, int world, int *bad, Fn f) {
+    for (int i = 0; i < world; ++i) {
+        bigclam_ctx *ctx = r[i];
+        *bad = i;
+        if (i > 0) CU(cudaSetDevice(ctx->device));
+        if (int rc = f(ctx)) return rc;
+    }
+    *bad = 0;
+    bigclam_ctx *ctx = r[0];
+    if (world > 1) CU(cudaSetDevice(ctx->device));
     return BIGCLAM_OK;
 }
 
-// One call of backtrackingLineSearchs.  The LLH it has to return is the PRE sum of the NEXT call, so
-// instead of a separate LLH pass the next call's whole step kernel is launched speculatively (same uset):
-// its PRE delivers this call's LLH, and when the next call arrives with the same uset its result is simply
-// committed (sumF update + buffer flip).  Any other entry point that touches the state drops the speculation.
-extern "C" int bigclam_step(bigclam_ctx *ctx, const uint8_t *node_mask, double *llh_out, int64_t *n_updated_out) {
-    if (ctx == nullptr) return BIGCLAM_EINVAL;
+// The finish_kernel of a round (launch_finish).
+struct RoundFinish {
+    long long kernel_index;
+    int variant;
+    double rel_tol;
+    bool apply, llh_is_final;
+};
+
+// One round of kernels: every rank's step (linesearch) or PRE-only kernel and the reduction behind it, then every
+// rank's combine and, given `fin`, its finish (without one the state stays as it is).  A rank's combine waits on device
+// flags for the other ranks' reductions, so nothing of the second pass may be queued in front of another rank's first
+// pass.  host_mask: the uset (n bytes), NULL for all nodes.
+static int group_round(bigclam_ctx *const *r, int world, bool linesearch, const uint8_t *host_mask, bool use_done,
+                       const RoundFinish *fin, int *bad) {
+    const int rc = each_rank(r, world, bad, [&](bigclam_ctx *ctx) {
+        if (host_mask != nullptr) CU(cudaMemcpyAsync(ctx->d_mask, host_mask, (size_t)ctx->n, cudaMemcpyHostToDevice, ctx->stream));
+        StepArgs a;
+        fill_args(ctx, a, linesearch, host_mask != nullptr ? ctx->d_mask : nullptr, use_done);
+        return timed_launch(ctx, a, linesearch);
+    });
+    if (rc != BIGCLAM_OK) return rc;
+    return each_rank(r, world, bad, [&](bigclam_ctx *ctx) {
+        if (int rx = launch_xreduce(ctx, use_done)) return rx;
+        if (fin == nullptr) return BIGCLAM_OK;
+        return launch_finish(ctx, fin->kernel_index, fin->variant, fin->rel_tol, fin->apply, fin->llh_is_final);
+    });
+}
+
+// Waits for every rank's stream.  check_pool: a rank whose row pool ran out reports BIGCLAM_ENOMEM.
+static int group_sync(bigclam_ctx *const *r, int world, bool check_pool, int *bad) {
+    return each_rank(r, world, bad, [&](bigclam_ctx *ctx) {
+        CU(cudaStreamSynchronize(ctx->stream));
+        return check_pool ? check_overflow(ctx) : BIGCLAM_OK;
+    });
+}
+
+// The LLH the last round left in the partials (the same bits on every rank), read on rank 0 once every rank is done.
+static int group_read_llh(bigclam_ctx *const *r, int world, bool check_pool, double *llh_out, int *bad) {
+    bigclam_ctx *ctx = r[0];
+    CU(cudaMemcpyAsync(ctx->h_pinned, ctx->d_partials + 2 * ctx->ld, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    if (int rc = group_sync(r, world, check_pool, bad)) return rc;
+    if (llh_out) *llh_out = ctx->h_pinned[0];
+    return BIGCLAM_OK;
+}
+
+static int group_llh(bigclam_ctx *const *r, int world, double *llh_out, int *bad) {
+    bigclam_ctx *ctx = r[0];
     CU(cudaSetDevice(ctx->device));
-    const bool speculate = (ctx->n_peers == 0);         // peers' replicas must never see uncommitted rows
+    if (int rc = each_rank(r, world, bad, reset_run_state)) return rc;
+    if (int rc = group_round(r, world, false, nullptr, false, nullptr, bad)) return rc;
+    // one context reads back the LLH alone; over several GPUs an exhausted row pool is reported here as well
+    return group_read_llh(r, world, world > 1, llh_out, bad);
+}
+
+// One call of backtrackingLineSearchs.  The LLH it has to return is the PRE sum of the NEXT call, so one context
+// without peers launches the next call's whole step kernel speculatively (same uset) instead of a separate LLH pass:
+// its PRE delivers this call's LLH, and when the next call arrives with the same uset its result is simply committed
+// (sumF update + buffer flip).  Any other entry point that touches the state drops the speculation.  Peers' replicas
+// must never see uncommitted rows: with peers, or over several GPUs, a PRE-only round gives the LLH.
+static int group_step(bigclam_ctx *const *r, int world, const uint8_t *node_mask, double *llh_out,
+                      int64_t *n_updated_out, int *bad) {
+    bigclam_ctx *ctx = r[0];
+    CU(cudaSetDevice(ctx->device));
+    const bool speculate = world == 1 && ctx->n_peers == 0;
     const bool null_mask = (node_mask == nullptr);
     const bool hit = speculate && ctx->spec_valid && ctx->spec_null_mask == null_mask &&
                      (null_mask || (ctx->spec_mask.size() == (size_t)ctx->n &&
                                     std::memcmp(ctx->spec_mask.data(), node_mask, (size_t)ctx->n) == 0));
-    int rc;
-    StepArgs a;
-    const uint8_t *d_mask = null_mask ? nullptr : ctx->d_mask;
-    if (!hit) {
-        rc = reset_run_state(ctx);
-        if (rc) return rc;
-    }
-    // the uset of this call always travels to the device (on a hit it equals what the speculative kernel used)
-    if (!null_mask) CU(cudaMemcpyAsync(ctx->d_mask, node_mask, (size_t)ctx->n, cudaMemcpyHostToDevice, ctx->stream));
-    if (!hit) {
-        fill_args(ctx, a, true, d_mask, false);
-        if (a.accepted != nullptr) a.accepted = ctx->d_accepted_spec;
-        rc = timed_launch(ctx, a, true);                   // PRE + LS + swap
-        if (rc) return rc;
-    } else {
+    if (hit) {
+        // the uset of this call still travels to the device: the next speculative kernel reads it
+        if (!null_mask) CU(cudaMemcpyAsync(ctx->d_mask, node_mask, (size_t)ctx->n, cudaMemcpyHostToDevice, ctx->stream));
         ctx->last_step_launches = 0;
         ctx->last_all_launches = 0;
+        // commit: sumF update (:192), n_updated, zero the partials; the speculative step's accepted[] becomes current
+        if (int rc = launch_finish(ctx, 0, 0, 0.0, true, false)) return rc;
+        std::swap(ctx->d_accepted, ctx->d_accepted_spec);
+    } else {
+        const RoundFinish commit{0, 0, 0.0, true, false};
+        if (int rc = each_rank(r, world, bad, reset_run_state)) return rc;
+        if (int rc = group_round(r, world, true, node_mask, false, &commit, bad)) return rc;   // PRE + LS + swap, commit
     }
-    // commit: sumF update (:192), n_updated, zero the partials; the step's accepted[] becomes current
-    rc = launch_finish(ctx, 0, 0, 0.0, true, false);
-    if (rc) return rc;
-    ctx->cur ^= 1;
-    ctx->dense_valid = false;
-    std::swap(ctx->d_accepted, ctx->d_accepted_spec);
+    for (int i = 0; i < world; ++i) {
+        r[i]->cur ^= 1;
+        r[i]->dense_valid = false;
+    }
     CU(cudaMemcpyAsync(ctx->h_pinned + 8, ctx->d_state, sizeof(RunState), cudaMemcpyDeviceToHost, ctx->stream));
     if (speculate) {
-        fill_args(ctx, a, true, d_mask, false);            // next call, speculatively: its PRE is this call's LLH
+        StepArgs a;
+        fill_args(ctx, a, true, null_mask ? nullptr : ctx->d_mask, false);   // next call, speculatively: its PRE is this call's LLH
         if (a.accepted != nullptr) a.accepted = ctx->d_accepted_spec;
-        rc = timed_launch(ctx, a, true);
-        if (rc) return rc;
+        if (int rc = timed_launch(ctx, a, true)) return rc;
         ctx->spec_valid = true;
         ctx->spec_null_mask = null_mask;
         if (!null_mask && !hit) ctx->spec_mask.assign(node_mask, node_mask + ctx->n);   // on a hit it is already equal
-    } else {
-        fill_args(ctx, a, false, nullptr, false);          // LLH with new F, new sumF (:196-219)
-        rc = timed_launch(ctx, a, false);
-        if (rc) return rc;
+    } else if (int rc = group_round(r, world, false, nullptr, false, nullptr, bad)) {   // LLH with new F, new sumF (:196-219)
+        return rc;
     }
-    CU(cudaMemcpyAsync(ctx->h_pinned, ctx->d_partials + 2 * ctx->ld, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    if (int ro = check_overflow(ctx)) return ro;
-    if (llh_out) *llh_out = ctx->h_pinned[0];
+    if (int rc = group_read_llh(r, world, true, llh_out, bad)) return rc;
     if (n_updated_out) *n_updated_out = reinterpret_cast<RunState *>(ctx->h_pinned + 8)->n_updated;
-    return collect_timing(ctx);
+    return each_rank(r, world, bad, collect_timing);
 }
 
-extern "C" int bigclam_run(bigclam_ctx *ctx, int32_t variant, double rel_tol, int64_t max_outer,
-                           double *llh_out, int64_t *calls_out, double *llh_trace, int64_t trace_cap) {
-    if (ctx == nullptr) return BIGCLAM_EINVAL;
-    if (variant != 2 && variant != 3 && variant != 4) return fail(ctx, BIGCLAM_EINVAL, "bigclam_run: variant must be 2, 3 or 4");
-    if (max_outer < 0 || trace_cap < 0) return fail(ctx, BIGCLAM_EINVAL, "bigclam_run: negative max_outer/trace_cap");
+// The outer loop (SGDFindC / MBSGD): every rank keeps the same device-side bookkeeping, since every rank sees the same
+// sums; the host reads rank 0's.
+static int group_run(bigclam_ctx *const *r, int world, int32_t variant, double rel_tol, int64_t max_outer,
+                     double *llh_out, int64_t *calls_out, double *llh_trace, int64_t trace_cap, int *bad) {
+    bigclam_ctx *ctx = r[0];
     CU(cudaSetDevice(ctx->device));
-    int rc = reset_run_state(ctx);
-    if (rc) return rc;
-    if (llh_trace != nullptr && trace_cap > 0) {
-        if (ctx->trace_cap < trace_cap) {
-            cudaFree(ctx->d_trace);
-            ctx->d_trace = nullptr;
-            ctx->trace_cap = 0;
-            CU(cudaMalloc(&ctx->d_trace, sizeof(double) * (size_t)trace_cap));
-            ctx->trace_cap = trace_cap;
-        }
+    if (int rc = each_rank(r, world, bad, reset_run_state)) return rc;
+    // the trace is written on rank 0 (the other ranks never have a trace buffer: trace_cap 0), into a buffer that only grows
+    if (llh_trace != nullptr && trace_cap > ctx->trace_cap) {
+        cudaFree(ctx->d_trace);
+        ctx->d_trace = nullptr;
+        ctx->trace_cap = 0;
+        CU(cudaMalloc(&ctx->d_trace, sizeof(double) * (size_t)trace_cap));
+        ctx->trace_cap = trace_cap;
     }
     const int64_t saved_cap = ctx->trace_cap;
-    if (llh_trace == nullptr) ctx->trace_cap = 0; else ctx->trace_cap = trace_cap;
+    ctx->trace_cap = (llh_trace != nullptr) ? trace_cap : 0;
 
     RunState *hst = reinterpret_cast<RunState *>(ctx->h_pinned + 8);
     const int start_cur = ctx->cur;
-    const int64_t batch = 8;       // the stream drains once per batch: the host reads the loop state and may re-cut the tiles
+    const int64_t batch = 8;       // the streams drain once per batch: the host reads the loop state and may re-cut the tiles
     int64_t c = 0;                 // step kernels enqueued so far (kernel c maps S_{c-1} -> S_c)
     bool done = false;
-    StepArgs a;
-    while (!done) {
-        int64_t todo = batch;
-        if (max_outer > 0) todo = std::min<int64_t>(batch, max_outer - c);
+    while (true) {
+        const int64_t todo = (max_outer > 0) ? std::min<int64_t>(batch, max_outer - c) : batch;
         for (int64_t i = 0; i < todo; ++i) {
             ++c;
-            ctx->cur = (start_cur + (int)((c - 1) & 1)) & 1;       // S_{c-1} lives in buffer (c-1)%2
-            fill_args(ctx, a, true, nullptr, true);
-            rc = timed_launch(ctx, a, true);
-            if (rc) return rc;
-            rc = launch_finish(ctx, c, variant, rel_tol, true, false);   // tests call c-1, builds sumF_c
-            if (rc) return rc;
+            const RoundFinish fin{c, variant, rel_tol, true, false};          // tests call c-1, builds sumF_c
+            if (int rc = group_round(r, world, true, nullptr, true, &fin, bad)) return rc;
+            for (int q = 0; q < world; ++q) r[q]->cur ^= 1;                 // cur: S_c
         }
         CU(cudaMemcpyAsync(hst, ctx->d_state, sizeof(RunState), cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
+        if (int rc = group_sync(r, world, false, bad)) return rc;
         if (hst->done) { done = true; break; }
         if (max_outer > 0 && c >= max_outer) break;
-        {   // the stream is idle: a good moment to re-cut the tiles when the rows have changed size a lot
-            const int keep = ctx->cur;
-            ctx->cur = (start_cur + (int)(c & 1)) & 1;            // S_c, the current state
-            const int rt = maybe_retile(ctx);
-            ctx->cur = keep;
-            if (rt) return rt;
-        }
+        // the stream is idle: a good moment to re-cut the tiles when the rows have changed size a lot.  The ranks of a
+        // multi-GPU handle keep the tiles they were cut with, so the nodes on their general paths stay the same.
+        if (world == 1)
+            if (int rt = maybe_retile(ctx)) return rt;
     }
-    int64_t calls;
-    if (done) {
-        calls = hst->conv_call;                                   // final state S_calls, untouched
-    } else {
-        calls = c;                                                // cut by max_outer: need LLH(S_c)
-        ctx->cur = (start_cur + (int)(c & 1)) & 1;
-        fill_args(ctx, a, false, nullptr, false);
-        rc = timed_launch(ctx, a, false);
-        if (rc) return rc;
-        rc = launch_finish(ctx, c, variant, rel_tol, false, true);
-        if (rc) return rc;
+    if (!done) {                   // cut by max_outer: need LLH(S_c)
+        const RoundFinish fin{c, variant, rel_tol, false, true};
+        if (int rc = group_round(r, world, false, nullptr, false, &fin, bad)) return rc;
         CU(cudaMemcpyAsync(hst, ctx->d_state, sizeof(RunState), cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
+        if (int rc = group_sync(r, world, false, bad)) return rc;
     }
-    ctx->cur = (start_cur + (int)(calls & 1)) & 1;
-    ctx->dense_valid = false;
-    invalidate_resets(ctx);
-    if (int ro = check_overflow(ctx)) return ro;
+    const int64_t calls = done ? hst->conv_call : c;                          // converged: final state S_calls, untouched
+    for (int i = 0; i < world; ++i) {
+        r[i]->cur = (start_cur + (int)(calls & 1)) & 1;
+        r[i]->dense_valid = false;
+        invalidate_resets(r[i]);
+    }
+    if (int rc = each_rank(r, world, bad, check_overflow)) return rc;         // the pools are checked once, at the end
     if (llh_out) *llh_out = hst->ret_llh;
     if (calls_out) *calls_out = calls;
     if (llh_trace != nullptr && trace_cap > 0) {
@@ -1356,7 +1392,29 @@ extern "C" int bigclam_run(bigclam_ctx *ctx, int32_t variant, double rel_tol, in
         if (cnt > 0) CU(cudaMemcpy(llh_trace, ctx->d_trace, sizeof(double) * (size_t)cnt, cudaMemcpyDeviceToHost));
     }
     ctx->trace_cap = saved_cap;
-    return collect_timing(ctx);
+    return each_rank(r, world, bad, collect_timing);
+}
+
+extern "C" int bigclam_loglikelihood(bigclam_ctx *ctx, double *llh_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    if (llh_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "bigclam_loglikelihood: llh_out is NULL");
+    int rank = 0;
+    return group_llh(&ctx, 1, llh_out, &rank);
+}
+
+extern "C" int bigclam_step(bigclam_ctx *ctx, const uint8_t *node_mask, double *llh_out, int64_t *n_updated_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    int rank = 0;
+    return group_step(&ctx, 1, node_mask, llh_out, n_updated_out, &rank);
+}
+
+extern "C" int bigclam_run(bigclam_ctx *ctx, int32_t variant, double rel_tol, int64_t max_outer,
+                           double *llh_out, int64_t *calls_out, double *llh_trace, int64_t trace_cap) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    if (variant != 2 && variant != 3 && variant != 4) return fail(ctx, BIGCLAM_EINVAL, "bigclam_run: variant must be 2, 3 or 4");
+    if (max_outer < 0 || trace_cap < 0) return fail(ctx, BIGCLAM_EINVAL, "bigclam_run: negative max_outer/trace_cap");
+    int rank = 0;
+    return group_run(&ctx, 1, variant, rel_tol, max_outer, llh_out, calls_out, llh_trace, trace_cap, &rank);
 }
 
 extern "C" int bigclam_get_kernel_time(bigclam_ctx *ctx, double *step_kernel_ms_sum, int64_t *step_kernel_launches,
@@ -1865,145 +1923,28 @@ extern "C" int bigclam_multi_get_F_csr(bigclam_multi *m, int64_t *indptr_out, in
     return BIGCLAM_OK;
 }
 
-// One kernel round over all ranks: every rank's step (or PRE-only) kernel and reduction first, then every rank's
-// combine + finish — a rank's combine waits on device flags for the other ranks' reductions, so nothing of the
-// second half may be queued in front of another rank's first half.
-static int multi_round(bigclam_multi *m, bool linesearch, const uint8_t *host_mask, bool use_done, long long kernel_index,
-                       int variant, double rel_tol, bool apply, bool llh_is_final) {
-    for (bigclam_ctx *c : m->r) {
-        if (cudaSetDevice(c->device) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "cudaSetDevice(%d) failed", c->device);
-        const uint8_t *d_mask = nullptr;
-        if (host_mask != nullptr) {
-            if (cudaMemcpyAsync(c->d_mask, host_mask, (size_t)c->n, cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
-                return mfail(m, BIGCLAM_ECUDA, "uset upload failed");
-            d_mask = c->d_mask;
-        }
-        StepArgs a;
-        fill_args(c, a, linesearch, d_mask, use_done);
-        MCALL(timed_launch(c, a, linesearch), c);
-    }
-    for (bigclam_ctx *c : m->r) {
-        if (cudaSetDevice(c->device) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "cudaSetDevice(%d) failed", c->device);
-        MCALL(launch_xreduce(c, use_done), c);
-        MCALL(launch_finish(c, kernel_index, variant, rel_tol, apply, llh_is_final), c);
-    }
-    return BIGCLAM_OK;
-}
-
-static int multi_sync(bigclam_multi *m) {
-    for (bigclam_ctx *c : m->r) {
-        if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess)
-            return mfail(m, BIGCLAM_ECUDA, "device %d: %s", c->device, cudaGetErrorString(cudaGetLastError()));
-        if (int ro = check_overflow(c)) return mfail_from(m, ro, c);
-    }
-    return BIGCLAM_OK;
-}
-
-// PRE-only round; the all-rank LLH lands in every rank's partials (finish with apply = 0 leaves the state alone)
-static int multi_llh(bigclam_multi *m, double *llh_out) {
-    for (bigclam_ctx *c : m->r) {
-        if (cudaSetDevice(c->device) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "cudaSetDevice(%d) failed", c->device);
-        StepArgs a;
-        fill_args(c, a, false, nullptr, false);
-        MCALL(timed_launch(c, a, false), c);
-    }
-    for (bigclam_ctx *c : m->r) {
-        if (cudaSetDevice(c->device) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "cudaSetDevice(%d) failed", c->device);
-        MCALL(launch_xreduce(c, false), c);
-    }
-    bigclam_ctx *c0 = m->r[0];
-    if (cudaSetDevice(c0->device) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "cudaSetDevice failed");
-    if (cudaMemcpyAsync(c0->h_pinned, c0->d_partials + 2 * c0->ld, sizeof(double), cudaMemcpyDeviceToHost, c0->stream) != cudaSuccess)
-        return mfail(m, BIGCLAM_ECUDA, "LLH download failed");
-    if (int rs = multi_sync(m)) return rs;
-    if (llh_out) *llh_out = c0->h_pinned[0];
-    return BIGCLAM_OK;
-}
-
 extern "C" int bigclam_multi_loglikelihood(bigclam_multi *m, double *llh_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
-    for (bigclam_ctx *c : m->r) { if (cudaSetDevice(c->device) == cudaSuccess) { int rc = reset_run_state(c); if (rc) return mfail_from(m, rc, c); } }
-    return multi_llh(m, llh_out);
-}
-
-// backtrackingLineSearchs(uset) over all GPUs: one step round, then a PRE-only round for the LLH it returns.
-extern "C" int bigclam_multi_step(bigclam_multi *m, const uint8_t *node_mask, double *llh_out, int64_t *n_updated_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    for (bigclam_ctx *c : m->r) { if (cudaSetDevice(c->device) == cudaSuccess) { int rc = reset_run_state(c); if (rc) return mfail_from(m, rc, c); } }
-    if (int rr = multi_round(m, true, node_mask, false, 0, 0, 0.0, true, false)) return rr;
-    for (bigclam_ctx *c : m->r) { c->cur ^= 1; c->dense_valid = false; }
-    bigclam_ctx *c0 = m->r[0];
-    cudaSetDevice(c0->device);
-    if (cudaMemcpyAsync(c0->h_pinned + 8, c0->d_state, sizeof(RunState), cudaMemcpyDeviceToHost, c0->stream) != cudaSuccess)
-        return mfail(m, BIGCLAM_ECUDA, "state download failed");
-    double llh = 0.0;
-    if (int rl = multi_llh(m, &llh)) return rl;
-    if (llh_out) *llh_out = llh;
-    if (n_updated_out) *n_updated_out = reinterpret_cast<RunState *>(c0->h_pinned + 8)->n_updated;
-    for (bigclam_ctx *c : m->r) { cudaSetDevice(c->device); collect_timing(c); }
+    int bad = 0;
+    if (int rc = group_llh(m->r.data(), m->world, llh_out, &bad)) return mfail_from(m, rc, m->r[(size_t)bad]);
     return BIGCLAM_OK;
 }
 
-// The outer loop (bigclam_run) over all GPUs: same device-side bookkeeping on every rank (they all see the same sums).
+extern "C" int bigclam_multi_step(bigclam_multi *m, const uint8_t *node_mask, double *llh_out, int64_t *n_updated_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    int bad = 0;
+    if (int rc = group_step(m->r.data(), m->world, node_mask, llh_out, n_updated_out, &bad)) return mfail_from(m, rc, m->r[(size_t)bad]);
+    return BIGCLAM_OK;
+}
+
 extern "C" int bigclam_multi_run(bigclam_multi *m, int32_t variant, double rel_tol, int64_t max_outer, double *llh_out,
                                  int64_t *calls_out, double *llh_trace, int64_t trace_cap) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     if (variant != 2 && variant != 3 && variant != 4) return mfail(m, BIGCLAM_EINVAL, "bigclam_multi_run: variant must be 2, 3 or 4");
     if (max_outer < 0 || trace_cap < 0) return mfail(m, BIGCLAM_EINVAL, "bigclam_multi_run: negative max_outer/trace_cap");
-    bigclam_ctx *c0 = m->r[0];
-    for (bigclam_ctx *c : m->r) {
-        if (cudaSetDevice(c->device) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "cudaSetDevice failed");
-        int rc = reset_run_state(c);
-        if (rc) return mfail_from(m, rc, c);
-        c->trace_cap = 0;
-    }
-    cudaSetDevice(c0->device);
-    if (llh_trace != nullptr && trace_cap > 0) {
-        cudaFree(c0->d_trace);
-        c0->d_trace = nullptr;
-        if (cudaMalloc(&c0->d_trace, sizeof(double) * (size_t)trace_cap) != cudaSuccess) return mfail(m, BIGCLAM_ENOMEM, "trace buffer");
-        c0->trace_cap = trace_cap;
-    }
-    RunState *hst = reinterpret_cast<RunState *>(c0->h_pinned + 8);
-    const int start_cur = c0->cur;
-    const int64_t batch = 8;
-    int64_t cdone = 0;
-    bool done = false;
-    while (!done) {
-        int64_t todo = batch;
-        if (max_outer > 0) todo = std::min<int64_t>(batch, max_outer - cdone);
-        for (int64_t i = 0; i < todo; ++i) {
-            ++cdone;
-            for (bigclam_ctx *c : m->r) c->cur = (start_cur + (int)((cdone - 1) & 1)) & 1;
-            if (int rr = multi_round(m, true, nullptr, true, cdone, variant, rel_tol, true, false)) return rr;
-        }
-        cudaSetDevice(c0->device);
-        if (cudaMemcpyAsync(hst, c0->d_state, sizeof(RunState), cudaMemcpyDeviceToHost, c0->stream) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "state download failed");
-        if (int rs = multi_sync(m)) return rs;
-        if (hst->done) { done = true; break; }
-        if (max_outer > 0 && cdone >= max_outer) break;
-    }
-    int64_t calls;
-    if (done) {
-        calls = hst->conv_call;
-    } else {
-        calls = cdone;
-        for (bigclam_ctx *c : m->r) c->cur = (start_cur + (int)(cdone & 1)) & 1;
-        if (int rr = multi_round(m, false, nullptr, false, cdone, variant, rel_tol, false, true)) return rr;
-        cudaSetDevice(c0->device);
-        if (cudaMemcpyAsync(hst, c0->d_state, sizeof(RunState), cudaMemcpyDeviceToHost, c0->stream) != cudaSuccess) return mfail(m, BIGCLAM_ECUDA, "state download failed");
-        if (int rs = multi_sync(m)) return rs;
-    }
-    for (bigclam_ctx *c : m->r) { c->cur = (start_cur + (int)(calls & 1)) & 1; c->dense_valid = false; invalidate_resets(c); }
-    if (llh_out) *llh_out = hst->ret_llh;
-    if (calls_out) *calls_out = calls;
-    if (llh_trace != nullptr && trace_cap > 0) {
-        const int64_t cnt = std::min<int64_t>(calls, trace_cap);
-        cudaSetDevice(c0->device);
-        if (cnt > 0 && cudaMemcpy(llh_trace, c0->d_trace, sizeof(double) * (size_t)cnt, cudaMemcpyDeviceToHost) != cudaSuccess)
-            return mfail(m, BIGCLAM_ECUDA, "trace download failed");
-    }
-    for (bigclam_ctx *c : m->r) { cudaSetDevice(c->device); collect_timing(c); }
+    int bad = 0;
+    if (int rc = group_run(m->r.data(), m->world, variant, rel_tol, max_outer, llh_out, calls_out, llh_trace, trace_cap, &bad))
+        return mfail_from(m, rc, m->r[(size_t)bad]);
     return BIGCLAM_OK;
 }
 
