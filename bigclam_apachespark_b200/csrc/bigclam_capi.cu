@@ -79,6 +79,8 @@ struct bigclam_ctx {
     int32_t *d_overflow = nullptr;
     int sp_grid = 0, sp_wpb = kSpWarps;
     size_t sp_smem = 0;
+    bool wide = false;                            // ld > 1024: the wide variant of the step kernel (bigclam_sparse.cuh), no tiles
+    unsigned char *d_wide_scratch = nullptr;      // its per-warp K-sized vectors: sp_grid * sp_wpb * sp_wide_warp_bytes(ld), zeroed
     bool dense_valid = true;       // d_F[cur] mirrors the sparse state (set_F; refreshed on demand by ensure_dense)
     uint64_t region_base8 = 0, region_cap8 = 0;   // this rank's part of every replica's output pool (multi-GPU)
     uint64_t *peer_hdr[2][7] = {{nullptr}};       // peers' headers / pools (both halves), IPC-mapped
@@ -217,7 +219,7 @@ static void free_ctx(bigclam_ctx *c) {
     cudaFree(c->d_hdr[0]); cudaFree(c->d_hdr[1]); cudaFree(c->d_pool[0]); cudaFree(c->d_pool[1]);
     cudaFree(c->d_pool_top); cudaFree(c->d_overflow);
     cudaFree(c->d_node_llh); cudaFree(c->d_dcnt); cudaFree(c->d_block_part); cudaFree(c->d_ticket);
-    cudaFree(c->d_tiles); cudaFree(c->d_tcol); cudaFree(c->d_stats);
+    cudaFree(c->d_tiles); cudaFree(c->d_tcol); cudaFree(c->d_stats); cudaFree(c->d_wide_scratch);
     if (c->x_ipc)
         for (int r = 0; r < c->x_world; ++r)
             if (r != c->x_rank) {
@@ -328,7 +330,7 @@ static int rebuild_sparse_lists(bigclam_ctx *ctx, const std::vector<NodeMeta> &m
     }
     // after the hubs: nodes above the tile budget go one per warp (general path), the rest in tiles of up to
     // kTlMaxNodes consecutive nodes with at most tile_edges edges
-    const int32_t budget = (ctx->nsteps <= 16) ? ctx->tile_edges : 0;
+    const int32_t budget = (ctx->nsteps <= 16 && !ctx->wide) ? ctx->tile_edges : 0;      // (wide rows: no tiles)
     int64_t pos = nh;
     while (pos < cnt && (budget <= 0 || meta[(size_t)pos].deg > budget)) ++pos;
     ctx->n_gen = (int32_t)(pos - nh);
@@ -472,8 +474,11 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
         return fail(ctx, BIGCLAM_EINVAL, "bigclam_create: need 0 < min_p < max_p < 1");
     if (!(params->min_f <= params->max_f)) return fail(ctx, BIGCLAM_EINVAL, "bigclam_create: min_f > max_f");
     const int32_t ld = (params->k + 3) & ~3;
-    if (ld > 1024)
-        return fail(ctx, BIGCLAM_EUNSUPPORTED, "bigclam_create: k = %d > 1024 not supported by this build", params->k);
+    const bool want_sparse = (params->flags & BIGCLAM_F_SPARSE_ROWS) != 0;
+    if (!want_sparse && ld > 1024)
+        return fail(ctx, BIGCLAM_EUNSUPPORTED, "bigclam_create: k = %d > 1024 not supported by the dense engine (BIGCLAM_F_SPARSE_ROWS: k <= %d)", params->k, kSpMaxK);
+    if (want_sparse && params->k > kSpMaxK)
+        return fail(ctx, BIGCLAM_EUNSUPPORTED, "bigclam_create: k = %d > %d, the limit of BIGCLAM_F_SPARSE_ROWS", params->k, kSpMaxK);
     const int64_t nnz = rowptr[n];
     if (rowptr[0] != 0 || nnz < 0) return fail(ctx, BIGCLAM_EINVAL, "bigclam_create: rowptr[0] != 0 or nnz < 0");
     for (int64_t u = 0; u < n; ++u)
@@ -534,29 +539,41 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
             return BIGCLAM_EUNSUPPORTED;
         }
         ctx->sparse = true;
-        ctx->sp_wpb = tl_warps_per_block(ld);
-        ctx->sp_smem = tl_block_smem_bytes(ld, ctx->sp_wpb);
-        int sbps = 0;
-        CUC(cudaFuncSetAttribute(tile_step_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
-        CUC(cudaFuncSetAttribute(tile_step_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
-        CUC(cudaFuncSetAttribute(tile_step_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
-        CUC(cudaFuncSetAttribute(tile_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+        ctx->wide = sp_wide(ld);
+        int sbps = 0, sb2 = 0;               // the grid must be resident for every variant (hub items wait for each other)
+        if (ctx->wide) {
+            ctx->sp_wpb = kTlWarps;
+            ctx->sp_smem = sp_wide_block_smem_bytes(ld, ctx->sp_wpb);
+            CUC(cudaFuncSetAttribute(tile_step_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaFuncSetAttribute(tile_step_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaFuncSetAttribute(tile_step_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaFuncSetAttribute(tile_step_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sbps, tile_step_kernel<true, true, true>, 32 * ctx->sp_wpb, ctx->sp_smem));
+            CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sb2, tile_step_kernel<false, false, true>, 32 * ctx->sp_wpb, ctx->sp_smem));
+        } else {
+            ctx->sp_wpb = tl_warps_per_block(ld);
+            ctx->sp_smem = tl_block_smem_bytes(ld, ctx->sp_wpb);
+            CUC(cudaFuncSetAttribute(tile_step_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaFuncSetAttribute(tile_step_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaFuncSetAttribute(tile_step_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaFuncSetAttribute(tile_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
+            CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sbps, tile_step_kernel<true, true>, 32 * ctx->sp_wpb, ctx->sp_smem));
+            CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sb2, tile_step_kernel<false, false>, 32 * ctx->sp_wpb, ctx->sp_smem));
+        }
         CUC(cudaFuncSetAttribute(reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * red_warps(ld) * (size_t)sp_ldp(ld))));
-        int sb2 = 0;                         // the grid must be resident for every variant (hub items wait for each other)
-        CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sbps, tile_step_kernel<true, true>, 32 * ctx->sp_wpb, ctx->sp_smem));
-        CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sb2, tile_step_kernel<false, false>, 32 * ctx->sp_wpb, ctx->sp_smem));
         sbps = std::min(sbps, sb2);
         if (sbps <= 0) {
             fail(nullptr, BIGCLAM_ECUDA, "bigclam_create: sparse kernel does not fit an SM (smem %zu B)", ctx->sp_smem);
             free_ctx(ctx);
             return BIGCLAM_ECUDA;
         }
-        sbps = std::min(sbps, tl_blocks_that_fit(ld, ctx->sp_wpb));
+        if (!ctx->wide) sbps = std::min(sbps, tl_blocks_that_fit(ld, ctx->sp_wpb));
         ctx->sp_grid = ctx->num_sms * sbps;
         ctx->h_work_init = 0;
         ctx->ls_exhaustive = (params->flags & BIGCLAM_F_LS_EXHAUSTIVE) != 0;
         if (const char *ev = std::getenv("BIGCLAM_LS_EXHAUSTIVE")) ctx->ls_exhaustive = std::atoi(ev) != 0;
         if (const char *ev = std::getenv("BIGCLAM_LS_PRUNE")) ctx->ls_level = std::max(1, std::min(2, std::atoi(ev)));
+        if (ctx->wide) ctx->ls_level = 1;            // (the wide variant has no bounds on the general path)
         if (const char *ev = std::getenv("BIGCLAM_TILE_EDGES")) ctx->tile_edges = std::max(0, std::min(kTlMaxEdges, std::atoi(ev)));
     } else {
         // dense rows (step_kernel): a persistent grid of kWarpsPerBlock-warp blocks, C2 double2 chunks of a row per lane
@@ -615,6 +632,11 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
     CUC(cudaMemset(ctx->d_accepted, 0xff, (size_t)n));
     CUC(cudaMemset(ctx->d_done, 0, sizeof(int32_t)));
     CUC(cudaMemset(ctx->d_state, 0, sizeof(RunState)));
+    if (ctx->wide) {               // (before the pools are sized from the free memory)
+        const size_t wbytes = (size_t)ctx->sp_grid * ctx->sp_wpb * sp_wide_warp_bytes(ld);
+        CUC(cudaMalloc(&ctx->d_wide_scratch, wbytes));
+        CUC(cudaMemset(ctx->d_wide_scratch, 0, wbytes));
+    }
     if (ctx->sparse) {
         // worst case: every row full (ld entries) — a step can then never overflow its pool.  When two such
         // pools do not fit in 80 % of the free memory, each pool gets 40 % of it and a step that runs out reports
@@ -745,7 +767,7 @@ static int check_overflow(bigclam_ctx *ctx) {
 // Sparse rows: the edge budget of a tile follows the rows' average size (the rows of a tile are staged in
 // kTlStage16 16-byte chunks of shared memory); called when F is set.  BIGCLAM_TILE_EDGES pins it instead.
 static int retile(bigclam_ctx *ctx, uint64_t words_used) {
-    if (!ctx->sparse || std::getenv("BIGCLAM_TILE_EDGES") != nullptr) return BIGCLAM_OK;
+    if (!ctx->sparse || ctx->wide || std::getenv("BIGCLAM_TILE_EDGES") != nullptr) return BIGCLAM_OK;
     std::vector<uint64_t> hdr((size_t)ctx->n);
     CU(cudaMemcpy(hdr.data(), ctx->d_hdr[ctx->cur], sizeof(uint64_t) * (size_t)ctx->n, cudaMemcpyDeviceToHost));
     const double nn = (double)std::max<int64_t>(1, ctx->n);
@@ -768,7 +790,7 @@ static int retile(bigclam_ctx *ctx, uint64_t words_used) {
 // The rows change size while the solver runs (they fill up on small-K problems): when the tiles were cut for rows
 // of a very different size, cut them again.  Call at a point where the stream is idle.
 static int maybe_retile(bigclam_ctx *ctx) {
-    if (!ctx->sparse || std::getenv("BIGCLAM_TILE_EDGES") != nullptr) return BIGCLAM_OK;
+    if (!ctx->sparse || ctx->wide || std::getenv("BIGCLAM_TILE_EDGES") != nullptr) return BIGCLAM_OK;
     // (1) tiles that keep falling back to the general path (too many active components / entries for the warp's
     //     buffers: small K, rows filling up) are cut smaller: the fallback costs three times the tile path
     unsigned int st[2] = {0u, 0u};
@@ -1079,9 +1101,15 @@ static int timed_launch(bigclam_ctx *ctx, const StepArgs &a, bool is_step) {
         sp.pr_xlo = std::nextafterf((float)a.x_lo, 0.0f);
         sp.pr_kinv = std::nextafterf((float)(1.0 / (1.0 - ctx->p.max_p)), INFINITY) * 1.000001f;
         sp.pr_cap = std::nextafterf((float)(a.t_hi - a.t_lo), INFINITY) * 1.000001f;
+        sp.wide_scratch = ctx->d_wide_scratch;
         const bool hub = a.n_hub_items > 0, push = sp.n_peers > 0;
         const int threads = 32 * ctx->sp_wpb;
-        if (hub && push) tile_step_kernel<true, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
+        if (ctx->wide) {
+            if (hub && push) tile_step_kernel<true, true, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
+            else if (hub) tile_step_kernel<false, true, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
+            else if (push) tile_step_kernel<true, false, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
+            else tile_step_kernel<false, false, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
+        } else if (hub && push) tile_step_kernel<true, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
         else if (hub) tile_step_kernel<false, true><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
         else if (push) tile_step_kernel<true, false><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);
         else tile_step_kernel<false, false><<<ctx->sp_grid, threads, ctx->sp_smem, ctx->stream>>>(a, sp);

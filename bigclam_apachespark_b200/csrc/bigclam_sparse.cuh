@@ -1,5 +1,5 @@
 // bigclam_sparse.cuh — the step (codes/bigclam4-7.scala:152-223) over SPARSE rows of F: layout, the general
-// one-warp-per-node path (any degree, any row length, K <= 1024) and the split-hub phases.  The tile path for
+// one-warp-per-node path (any degree, any row length, K <= 16384) and the split-hub phases.  The tile path for
 // small nodes and the kernels themselves are in bigclam_tile.cuh.
 //
 // Why: the reference keeps F as Breeze sparse vectors (`BSV[Double]`, bigclam4-7.scala:97-104) because the rows
@@ -33,7 +33,16 @@
 //   SWAP  the accepted candidate's non-zeros are compacted (ascending) into the staging buffer, a block is
 //         taken from the output pool, the row, its delta block and its header are written.
 //
-// Limits: ld <= 1024, MIN_F_ == 0.
+// Wide rows (ld > 1024, the `kWide` variant of the step kernel): the K-sized vectors of a warp (fu_d, g_d, the entry
+// buffer, aidx) no longer fit shared memory, so they live in the warp's slice of a global scratch that the context
+// allocates and zeroes once (sp_wide_warp_bytes); sumF is read from global memory.  Every node is a general-path item
+// (no tiles).  The per-node passes cover only the components the node TOUCHES (its own non-zeros and its neighbours'),
+// kept in a per-warp bitmask in shared memory: the gradient scan, the active list and the clears visit its set bits.
+// An untouched component has fu = 0 and gradient -sumF_c <= 0: it is inactive and enters |g|^2 through
+// S2_all - sum_touched sumF_c^2 (the identity of the tile path).  The line-search bounds of the general path
+// (BIGCLAM_LS_PRUNE=2) are not compiled into the wide variant.  The scratch is all zero between nodes and launches.
+//
+// Limits: ld <= 1024 (ld <= kSpMaxK with the wide variant), MIN_F_ == 0.
 #pragma once
 #include "bigclam_kernels.cuh"
 
@@ -102,6 +111,7 @@ struct SparseArgs {
     // 1 = bounds on the tile path only, 2 = on the general path too
     int32_t ls_prune;
     float pr_xlo, pr_kinv, pr_cap;     // x_lo rounded down, 1 / (1 - MAX_P_) and S_hi - S_lo rounded up
+    unsigned char *wide_scratch;       // wide rows: sp_wide_warp_bytes(ld) per resident warp, all zero between launches
 };
 
 // The dense per-warp vectors are padded to a multiple of 32 components (zeros: a padding component has
@@ -111,6 +121,24 @@ __host__ __device__ inline int sp_ldp(int ld) { return (ld + 31) & ~31; }
 //   fu_d[ldp] | g_d[ldp] | ent_val[E] | ent_idx[E] u16 | aidx[max(ld, 256)] u16 | poff[40] u16 | cbal[32] u32 | ccum[32] u16
 __host__ __device__ inline size_t sp_gen_warp_bytes(int ld) {
     return sizeof(double) * 2 * (size_t)sp_ldp(ld) + (size_t)sp_entries(ld) * 10 + 2 * (size_t)(ld > 256 ? ld : 256) + 2 * 40 + 4 * 32 + 2 * 32;
+}
+// wide rows: the largest K of a sparse-row context (component ids, dcnt, poff and aidx are uint16), and the ld above
+// which the wide variant runs
+constexpr int kSpMaxK = 16384;
+constexpr int kSpWideLd = 1024;
+__host__ __device__ inline bool sp_wide(int ld) { return ld > kSpWideLd; }
+// wide rows, per warp: global scratch  fu_d[ldp] | g_d[ldp] | ent_val[E] | ent_idx[E] u16 | aidx[ld] u16
+__host__ __device__ inline size_t sp_wide_warp_bytes(int ld) {
+    return (sizeof(double) * 2 * (size_t)sp_ldp(ld) + (size_t)sp_entries(ld) * 10 + 2 * (size_t)ld + 15) & ~(size_t)15;
+}
+// ... and shared memory  tmask[ldp / 32] u32 | cbal[E / 32] u32 | poff[40] u16 | ccum[E / 32] u16  (a chunk of the entry
+// buffer may hold E = ld entries: compact_active keeps one ballot per 32 of them)
+__host__ __device__ inline size_t sp_wide_smem_warp_bytes(int ld) {
+    return (4 * (size_t)(sp_ldp(ld) / 32) + 6 * (size_t)(sp_ldp(sp_entries(ld)) / 32) + 2 * 40 + 15) & ~(size_t)15;
+}
+// block: steps[kMaxSteps] | wpb x warp region
+__host__ __device__ inline size_t sp_wide_block_smem_bytes(int ld, int wpb) {
+    return sizeof(double) * kMaxSteps + (size_t)wpb * sp_wide_smem_warp_bytes(ld);
 }
 
 // Split hubs.  A node whose neighbour list is long enough to dominate a launch when one warp walks it is split
@@ -174,21 +202,46 @@ __device__ __forceinline__ void ls_code_near(double x, double x_lo, double En, f
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The general path: everything one warp needs to process one node (or one hub item).
+// The general path: everything one warp needs to process one node (or one hub item).  kWide: wide rows (see the
+// header comment): K-sized vectors in global scratch, sumF in global memory, touched-only per-node passes.
+template <bool kWide>
 struct SpGen {
     // launch-wide
     const StepArgs *a;
     const SparseArgs *sp;
     const double *s_steps;
-    const double *s_sumF;
+    const double *s_sumF;            // (wide rows: the global sumF)
     const float *s_lns;              // upper bounds of ln(step size), 16 values (line search by bounds)
+    double S2_all;                   // wide rows: sum_c sumF_c^2 (fixed order)
     EdgeConst ec;
     // per warp
     double *fu_d, *g_d, *ent_val;
     unsigned short *ent_idx, *aidx, *poff, *ccum;
     unsigned int *cbal;
+    unsigned int *tmask;             // wide rows: the components the current node touches, one bit each
     int lane, ld, ldp, ecap;
     unsigned lt_mask;
+
+    // wide rows: the K-sized vectors in the warp's slice `gbase` of the global scratch, the rest in shared memory
+    __device__ __forceinline__ void carve_wide(unsigned char *gbase, unsigned char *sbase, int ld_, int lane_) {
+        ld = ld_;
+        ldp = sp_ldp(ld_);
+        ecap = sp_entries(ld_);
+        lane = lane_;
+        lt_mask = (1u << lane_) - 1u;
+        fu_d = reinterpret_cast<double *>(gbase);
+        g_d = fu_d + ldp;
+        ent_val = g_d + ldp;
+        ent_idx = reinterpret_cast<unsigned short *>(ent_val + ecap);
+        aidx = ent_idx + ecap;
+        tmask = reinterpret_cast<unsigned int *>(sbase);
+        cbal = tmask + ldp / 32;
+        poff = reinterpret_cast<unsigned short *>(cbal + sp_ldp(ecap) / 32);
+        ccum = poff + 40;
+    }
+    __device__ __forceinline__ void touch(int c) {
+        if constexpr (kWide) atomicOr(tmask + (c >> 5), 1u << (c & 31));
+    }
 
     __device__ __forceinline__ void carve(unsigned char *wbase, int ld_, int lane_) {
         ld = ld_;
@@ -284,6 +337,7 @@ struct SpGen {
                     for (int i = pe + lane; i < pn; i += 32) {
                         const int c = ent_idx[i];
                         g_d[c] = fma(we, ent_val[i], g_d[c]);
+                        touch(c);
                     }
                     __syncwarp();
                 }
@@ -305,7 +359,7 @@ struct SpGen {
         for (int c0 = 0; c0 < ldp; c0 += 32) {          // (padding components: f = g = 0, inactive)
             const int c = c0 + lane;
             const double f = fu_d[c];
-            const double g = (g_d[c] - s_sumF[c]) + f;
+            const double g = (g_d[c] - ((kWide && c >= ld) ? 0.0 : s_sumF[c])) + f;     // (the global sumF has ld entries)
             g_d[c] = g;
             G2 = fma(g, g, G2);
             const bool act = (f > 0.0 || g > 0.0);
@@ -320,6 +374,80 @@ struct SpGen {
         need_hi = __any_sync(0xffffffffu, hi_lane);
         __syncwarp();
         return G2;
+    }
+    // Wide rows: the same over the TOUCHED components only (ascending, from the bitmask); the others are inactive and
+    // enter |g|^2 through S2_all - sum_touched sumF_c^2.  The touched list is built in aidx and compacted in place to
+    // the active list.
+    __device__ __forceinline__ double scan_touched(int &m, bool &need_hi) {
+        const int W = ldp >> 5;
+        int nt = 0;
+#pragma unroll 1
+        for (int w0 = 0; w0 < W; w0 += 32) {
+            const int w = w0 + lane;
+            unsigned bits = (w < W) ? tmask[w] : 0u;
+            const int pc = __popc(bits);
+            int incl = pc;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            int p = nt + incl - pc;
+            while (bits) {
+                aidx[p++] = (unsigned short)(32 * w + __ffs(bits) - 1);
+                bits &= bits - 1u;
+            }
+            nt += __shfl_sync(0xffffffffu, incl, 31);
+        }
+        __syncwarp();
+        double G2 = 0.0, SF2 = 0.0;
+        bool hi_lane = false;
+        m = 0;
+        const double max_f = a->max_f;
+#pragma unroll 1
+        for (int t0 = 0; t0 < nt; t0 += 32) {
+            const int t = t0 + lane;
+            const bool ok = t < nt;
+            const int c = ok ? (int)aidx[t] : 0;
+            double f = 0.0, g = 0.0;
+            if (ok) {
+                const double sf = s_sumF[c];
+                f = fu_d[c];
+                g = (g_d[c] - sf) + f;
+                g_d[c] = g;
+                G2 = fma(g, g, G2);
+                SF2 = fma(sf, sf, SF2);
+            }
+            const bool act = ok && (f > 0.0 || g > 0.0);
+            const unsigned bal = __ballot_sync(0xffffffffu, act);
+            __syncwarp();                                 // this round's reads are done; the writes land at or below them
+            if (act) {
+                aidx[m + __popc(bal & lt_mask)] = (unsigned short)c;
+                hi_lane |= (f + g > max_f);
+            }
+            m += __popc(bal);
+        }
+        G2 = warp_sum(G2);
+        SF2 = warp_sum(SF2);
+        need_hi = __any_sync(0xffffffffu, hi_lane);
+        __syncwarp();
+        return (S2_all - SF2) + G2;
+    }
+    // Wide rows: g_d of the touched components back to zero (when it was written) and the bitmask cleared.
+    __device__ __forceinline__ void clear_touched(bool clear_g) {
+        const int W = ldp >> 5;
+#pragma unroll 1
+        for (int w = lane; w < W; w += 32) {
+            unsigned bits = tmask[w];
+            if (bits == 0u) continue;
+            if (clear_g)
+                while (bits) {
+                    g_d[32 * w + __ffs(bits) - 1] = 0.0;
+                    bits &= bits - 1u;
+                }
+            tmask[w] = 0u;
+        }
+        __syncwarp();
     }
     // The staged entries of `ne` rows shrink, in place, to those on ACTIVE components (fu > 0 or grad > 0): only
     // they can contribute to a candidate's dot.  Order inside a row is kept, poff is rewritten.
@@ -518,6 +646,7 @@ struct SpGen {
             const double v = __ldg(uval + i);
             const int c = __ldg(uidx + i);
             fu_d[c] = v;
+            touch(c);
             fusf = fma(v, s_sumF[c], fusf);
             fufu = fma(v, v, fufu);
         }
@@ -645,10 +774,13 @@ struct SpGen {
         int jstar = -1, m = 0;
         if (want_ls) {
             bool need_hi;
-            const double G2 = scan_gradient(m, need_hi);
+            double G2;
+            if constexpr (kWide) G2 = scan_touched(m, need_hi);
+            else G2 = scan_gradient(m, need_hi);
             // ---------------- LS (:172-182): only if the bounds leave a candidate that can pass ----------------
             unsigned surv = 0xffffu;
-            if (BIGCLAM_GEN_BOUNDS && sp->ls_prune > 1 && nsteps <= 16) surv = bound_mask(colp, deg, m, G2, llh_u, fusf, fufu, nchunks == 1 ? ne_last : 0);
+            if constexpr (!kWide)           // (wide rows: no bounds on the general path)
+                if (BIGCLAM_GEN_BOUNDS && sp->ls_prune > 1 && nsteps <= 16) surv = bound_mask(colp, deg, m, G2, llh_u, fusf, fufu, nchunks == 1 ? ne_last : 0);
             if (sp->stats != nullptr && lane == 0) {
                 atomicAdd(sp->stats + 3, 1u);
                 if (surv != 0u) atomicAdd(sp->stats + 2, 1u);
@@ -673,9 +805,13 @@ struct SpGen {
         __syncwarp();
 #pragma unroll 1
         for (int i = lane; i < cu; i += 32) fu_d[__ldg(uidx + i)] = 0.0;
-        if (want_ls)
+        if constexpr (kWide) {
+            clear_touched(want_ls);
+        } else {
+            if (want_ls)
 #pragma unroll 1
-            for (int c = lane; c < ldp; c += 32) g_d[c] = 0.0;
+                for (int c = lane; c < ldp; c += 32) g_d[c] = 0.0;
+        }
         __syncwarp();
     }
 
@@ -787,6 +923,10 @@ struct SpGen {
         __syncwarp();
 #pragma unroll 1
         for (int i = lane; i < cu; i += 32) fu_d[__ldg(uidx + i)] = 0.0;
+        if constexpr (kWide) {            // (the hub phases loop over all components: only the bitmask is left to clear)
+#pragma unroll 1
+            for (int w = lane; w < (ldp >> 5); w += 32) tmask[w] = 0u;
+        }
         __syncwarp();
     }
 };

@@ -1026,13 +1026,70 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
     }
 };
 
-// kPush: multi-GPU launch, the peers' replicas are written too; kHub: the launch has split hubs.  Both are
-// compile-time so that the plain single-GPU kernel carries none of that code.
+// Wide rows (ld > 1024, bigclam_sparse.cuh): no tiles, every node with edges on the general path (hubs split as
+// usual), the K-sized vectors in the warp's slice of sp.wide_scratch, sumF read from global memory.
 template <bool kPush, bool kHub>
+__device__ __forceinline__ void wide_step(const StepArgs &a, const SparseArgs &sp, unsigned char *smem_raw) {
+    const int ld = a.ld;
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    double *s_steps = reinterpret_cast<double *>(smem_raw);
+#pragma unroll 1
+    for (int i = threadIdx.x; i < kMaxSteps; i += (int)blockDim.x) s_steps[i] = a.steps[i];
+    __syncthreads();
+    // S2_all = sum_c sumF_c^2 in a fixed order (every warp computes the same bits)
+    double S2 = 0.0;
+#pragma unroll 1
+    for (int c = lane; c < ld; c += 32) S2 = fma(a.sumF[c], a.sumF[c], S2);
+    S2 = warp_sum(S2);
+
+    SpGen<true> G;
+    G.a = &a;
+    G.sp = &sp;
+    G.s_steps = s_steps;
+    G.s_sumF = a.sumF;
+    G.s_lns = nullptr;
+    G.S2_all = S2;
+    G.ec = {a.x_lo, a.x_hi, a.t_lo, a.t_hi, a.w_lo, a.w_hi};
+    const size_t gw = (size_t)blockIdx.x * (blockDim.x >> 5) + (size_t)wib;
+    G.carve_wide(sp.wide_scratch + gw * sp_wide_warp_bytes(ld),
+                 smem_raw + sizeof(double) * kMaxSteps + (size_t)wib * sp_wide_smem_warp_bytes(ld), ld, lane);
+#pragma unroll 1
+    for (int w = lane; w < G.ldp / 32; w += 32) G.tmask[w] = 0u;
+    __syncwarp();
+
+    if constexpr (kHub) {
+        for (;;) {
+            unsigned int it = 0;
+            if (lane == 0) it = atomicAdd(sp.hub_work, 1u);
+            it = __shfl_sync(0xffffffffu, it, 0);
+            if (it >= (unsigned int)a.n_hub_items) break;
+            G.template hub_item<kPush>(a.hub_items[it]);
+        }
+    }
+
+    unsigned int item = 0;
+    if (lane == 0) item = atomicAdd(a.work_counter, 1u);
+    item = __shfl_sync(0xffffffffu, item, 0);
+    while (item < (unsigned int)sp.n_gen) {
+        unsigned int nxt = 0;
+        if (lane == 0) nxt = atomicAdd(a.work_counter, 1u);
+        const NodeMeta nm = a.meta[(int64_t)a.n_hubs + item];
+        G.template node<kPush>(nm.u, nm.deg, a.col + nm.e0);
+        item = __shfl_sync(0xffffffffu, nxt, 0);
+    }
+}
+
+// kPush: multi-GPU launch, the peers' replicas are written too; kHub: the launch has split hubs; kWide: wide rows
+// (ld > 1024, see wide_step).  All three are compile-time so that the plain single-GPU kernel carries none of that code.
+template <bool kPush, bool kHub, bool kWide = false>
 __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(const __grid_constant__ StepArgs a, const __grid_constant__ SparseArgs sp) {
     if (a.done_flag != nullptr && *a.done_flag != 0) return;
 
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    if constexpr (kWide) {
+        wide_step<kPush, kHub>(a, sp, smem_raw);
+        return;
+    }
     const int ld = a.ld;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nthreads = (int)blockDim.x;
@@ -1058,7 +1115,7 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     for (int c = lane; c < ldp; c += 32) S2 = fma(s_sumF[c], s_sumF[c], S2);
     S2 = warp_sum(S2);
 
-    SpGen G;
+    SpGen<false> G;
     G.a = &a;
     G.sp = &sp;
     G.s_steps = s_steps;
@@ -1157,7 +1214,13 @@ struct ReduceArgs {
     unsigned long long seq;
 };
 constexpr int kRedWarps = 32;      // at most; every warp keeps a dense vector of ldp doubles in shared memory: wide rows run fewer warps
-inline int red_warps(int ld) { const int ldp = sp_ldp(ld); return ldp <= 384 ? 32 : ldp <= 768 ? 16 : 8; }
+// (above ld = 1024: as many warps as 224 KB hold, 8 at most, 1 at K = 16384)
+inline int red_warps(int ld) {
+    const int ldp = sp_ldp(ld);
+    if (ldp <= 1024) return ldp <= 384 ? 32 : ldp <= 768 ? 16 : 8;
+    const int w = (int)((size_t)224 * 1024 / (sizeof(double) * (size_t)ldp));
+    return w < 1 ? 1 : w > 8 ? 8 : w;
+}
 
 __global__ void __launch_bounds__(kRedWarps * 32) reduce_kernel(const ReduceArgs r) {
     if (r.done_flag != nullptr && *r.done_flag != 0) return;

@@ -86,7 +86,7 @@ class BigClam:
         self.MIN_P_, self.MAX_P_, self.MIN_F_, self.MAX_F_ = 0.0001, 0.9999, 0.0, 1000.0   # :40-43
         self.device = device
         self.flags = (_lib.F_TIME_KERNELS if time_kernels else 0) | (_lib.F_RECORD_ACCEPTED if record_accepted else 0)
-        if sparse_rows:       # F as sparse rows on the device (the reference's BSV[Double]); K <= 256, one GPU
+        if sparse_rows:       # F as sparse rows on the device (the reference's BSV[Double]); K <= 16384
             self.flags |= _lib.F_SPARSE_ROWS
         if exhaustive_linesearch:     # evaluate every candidate of every node (no bounds), like the reference's cartesian (:172-181)
             self.flags |= _lib.F_LS_EXHAUSTIVE
@@ -131,7 +131,8 @@ class BigClam:
         check(lib.bigclam_default_params(C.byref(p), self.K))
         p.max_inter, p.alpha, p.beta = self.MaxInter, self.alpha, self.beta
         p.min_p, p.max_p, p.min_f, p.max_f = self.MIN_P_, self.MAX_P_, self.MIN_F_, self.MAX_F_
-        p.device, p.flags = self.device, self.flags
+        # above K = 1024 only sparse rows hold F (the dense engine stops there): a K sweep crosses 1024 on its own
+        p.device, p.flags = self.device, self.flags | (_lib.F_SPARSE_ROWS if self.K > 1024 else 0)
         ctx = C.c_void_p()
         if self.numGPUs > 1:
             devs = None

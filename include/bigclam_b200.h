@@ -55,9 +55,13 @@ typedef struct {
 #define BIGCLAM_F_TIME_KERNELS   1   /* record CUDA events around every step-kernel launch */
 #define BIGCLAM_F_RECORD_ACCEPTED 2  /* keep the accepted step index per node (diagnostics/tests) */
 #define BIGCLAM_F_SPARSE_ROWS     4  /* keep F as sparse rows on the device (like the reference's BSV[Double],
-                                        bigclam4-7.scala:97-104): k <= 1024, min_f == 0, n < 2^28.  The dense entry
+                                        bigclam4-7.scala:97-104): k <= 16384, min_f == 0, n < 2^28.  The dense entry
                                         points still work (bigclam_set_F / bigclam_get_F convert on the device);
-                                        bigclam_set_F_csr / bigclam_get_F_csr never build a dense image. */
+                                        bigclam_set_F_csr / bigclam_get_F_csr never build a dense image.
+                                        Above k = 1024 the step runs a wide variant: no tiles (bigclam_get_tile_stats
+                                        reports n_tiles == 0), the per-warp K-sized vectors in a device scratch of
+                                        (resident warps x 28 bytes x k), per-node passes over the touched components
+                                        only, and no line-search bounds on the general path (BIGCLAM_LS_PRUNE=2). */
 
 #define BIGCLAM_F_LS_EXHAUSTIVE   8  /* sparse rows: evaluate all max_inter+1 candidates of every node like the reference
                                         does (bigclam4-7.scala:172-181).  Default: a candidate that a bound on the node's
@@ -76,6 +80,8 @@ int bigclam_step_sizes(double beta, int32_t max_inter, double *out);
  * buffer, sumF.  rowptr has n+1 entries, col has rowptr[n] entries in [0,n); neighbour lists are
  * taken as given (multiplicity and order preserved, like collectNeighborIds(Either)).
  * Replaces: Neightborbc broadcast (:51) and the per-call Fbc broadcast (:154).
+ * Limits on k: 1024 for dense rows, 16384 with BIGCLAM_F_SPARSE_ROWS; above them BIGCLAM_EUNSUPPORTED (checked
+ * before any device is touched).
  */
 int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowptr, const int32_t *col,
                    const bigclam_params *params);

@@ -112,7 +112,7 @@ public:
         p.beta = beta;
         p.max_inter = MaxInter;
         p.device = device_;
-        p.flags = flags_;
+        p.flags = flags_ | (K > 1024 ? BIGCLAM_F_SPARSE_ROWS : 0);      // (the dense engine stops at K = 1024)
         if (world_ > 1) {
             const int rc = bigclam_multi_create(&multi_, n_, rowptr_.data(), col_.data(), &p, world_, nullptr);
             if (rc != BIGCLAM_OK) throw Error(rc, str(bigclam_multi_last_error(nullptr)));
