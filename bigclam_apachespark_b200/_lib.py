@@ -118,6 +118,10 @@ SIGNATURES = {
     "bigclam_graph_read_edgelist": (C.c_int, [C.c_char_p, _i32, C.POINTER(Graph), C.c_char_p, _i64]),
     "bigclam_graph_free": (None, [C.POINTER(Graph)]),
     "bigclam_extract": (C.c_int, [_vp, _dbl, _vp, _vp]),
+    "bigclam_pair_affinity": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp]),
+    "bigclam_recommend": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "bigclam_multi_pair_affinity": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp]),
+    "bigclam_multi_recommend": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "bigclam_conductance_seeds": (C.c_int, [_i64, _vp, _vp, _vp, _vp, _pi64]),
     "bigclam_conductance_seeds_gpu": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _vp, _pi64]),
     "bigclam_init_neighbor_com_F": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _i64, _i32, C.c_uint64, _vp]),

@@ -1722,6 +1722,157 @@ extern "C" int bigclam_extract(bigclam_ctx *ctx, double delta, uint8_t *member_o
 }
 
 // ------------------------------------------------------------------------------------------------
+// Edge probabilities and link recommendations (bigclam_sparse.cuh, pair_x): read the current F where it lives (the
+// sparse rows, or the dense buffer of a dense context) on the context's stream.  They change no state: a speculative
+// step queued in front of them reads the same buffer and writes the other one.
+
+// A device buffer that is freed when it goes out of scope (the CU early returns).
+template <class T>
+struct DevBuf {
+    T *p = nullptr;
+    size_t cap = 0;
+    ~DevBuf() { cudaFree(p); }
+    cudaError_t reserve(size_t count) {
+        if (count <= cap) return cudaSuccess;
+        cudaFree(p);
+        p = nullptr;
+        cap = 0;
+        cudaError_t e = cudaMalloc(&p, sizeof(T) * std::max<size_t>(1, count));
+        if (e == cudaSuccess) cap = count;
+        else (void)cudaGetLastError();
+        return e;
+    }
+};
+
+static RowSrc row_src(const bigclam_ctx *ctx) {
+    RowSrc s{};
+    if (ctx->sparse) {
+        s.hdr = ctx->d_hdr[ctx->cur];
+        s.pool = ctx->d_pool[ctx->cur];
+    } else {
+        s.F = ctx->d_F[ctx->cur];
+    }
+    s.k = ctx->p.k;
+    s.ld = ctx->ld;
+    return s;
+}
+
+static int check_ids(bigclam_ctx *ctx, const char *what, const char *name, const int32_t *ids, int64_t count) {
+    for (int64_t i = 0; i < count; ++i)
+        if (ids[i] < 0 || ids[i] >= ctx->n)
+            return fail(ctx, BIGCLAM_EINVAL, "%s: %s[%lld] = %d is outside [0, %lld)", what, name, (long long)i, ids[i], (long long)ctx->n);
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_pair_affinity(bigclam_ctx *ctx, const int32_t *u, const int32_t *v, int64_t count, double *x_out, double *p_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_pair_affinity";
+    if (count < 0) return fail(ctx, BIGCLAM_EINVAL, "%s: count < 0", what);
+    if (count == 0) return BIGCLAM_OK;
+    if (u == nullptr || v == nullptr || x_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: u, v or x_out is NULL", what);
+    if (int rc = check_ids(ctx, what, "u", u, count)) return rc;
+    if (int rc = check_ids(ctx, what, "v", v, count)) return rc;
+    CU(cudaSetDevice(ctx->device));
+    const RowSrc s = row_src(ctx);
+    const PairConst pc{ctx->p.min_p, ctx->p.max_p, -std::log(ctx->p.max_p) * (1.0 - 1e-12), -std::log(ctx->p.min_p) * (1.0 + 1e-12)};
+    const int64_t chunk = std::min<int64_t>(count, (int64_t)1 << 22);      // pairs per transfer
+    DevBuf<int32_t> du, dv;
+    DevBuf<double> dx, dp;
+    CU(du.reserve((size_t)chunk));
+    CU(dv.reserve((size_t)chunk));
+    CU(dx.reserve((size_t)chunk));
+    if (p_out != nullptr) CU(dp.reserve((size_t)chunk));
+    for (int64_t c0 = 0; c0 < count; c0 += chunk) {
+        const int64_t nc = std::min(chunk, count - c0);
+        CU(cudaMemcpyAsync(du.p, u + c0, sizeof(int32_t) * (size_t)nc, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dv.p, v + c0, sizeof(int32_t) * (size_t)nc, cudaMemcpyHostToDevice, ctx->stream));
+        pair_affinity_kernel<<<(unsigned)((nc + 127) / 128), 128, 0, ctx->stream>>>(s, pc, du.p, dv.p, nc, dx.p, p_out ? dp.p : nullptr);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(x_out + c0, dx.p, sizeof(double) * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+        if (p_out != nullptr) CU(cudaMemcpyAsync(p_out + c0, dp.p, sizeof(double) * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_recommend(bigclam_ctx *ctx, const int32_t *nodes, int64_t count, int32_t m, int32_t *v_out, double *x_out,
+                                 int32_t *found_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_recommend";
+    if (count < 0) return fail(ctx, BIGCLAM_EINVAL, "%s: count < 0", what);
+    if (m < 1) return fail(ctx, BIGCLAM_EINVAL, "%s: m = %d, must be >= 1", what, m);
+    if (nodes == nullptr && count != ctx->n) return fail(ctx, BIGCLAM_EINVAL, "%s: nodes is NULL (all nodes) but count != n", what);
+    if (count == 0) return BIGCLAM_OK;
+    if (v_out == nullptr || x_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: v_out or x_out is NULL", what);
+    if (nodes != nullptr)
+        if (int rc = check_ids(ctx, what, "nodes", nodes, count)) return rc;
+    CU(cudaSetDevice(ctx->device));
+    const RowSrc s = row_src(ctx);
+    // scratch bound: the smaller of 1 GiB and 10 % of the free memory, for the two-hop keys of a batch of nodes; a node
+    // whose list alone is longer gets a batch of its own with scratch sized for it
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    const int64_t budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    const int64_t budget_keys = std::max<int64_t>(1, budget / (int64_t)sizeof(uint32_t));
+    const int64_t Q = std::max<int64_t>(1, std::min<int64_t>({count, (int64_t)1 << 16, budget / (12 * (int64_t)m + 64)}));   // nodes per chunk
+    DevBuf<int32_t> dq, dv, dfound;
+    DevBuf<int64_t> dcnt, doff;
+    DevBuf<double> dx;
+    DevBuf<uint32_t> keys;
+    CU(dq.reserve((size_t)Q));
+    CU(dcnt.reserve((size_t)Q));
+    CU(doff.reserve((size_t)Q + 1));
+    CU(dv.reserve((size_t)Q * m));
+    CU(dx.reserve((size_t)Q * m));
+    CU(dfound.reserve((size_t)Q));
+    std::vector<int32_t> hq((size_t)Q);
+    std::vector<int64_t> hcnt((size_t)Q), hoff((size_t)Q + 1);
+    const int wpb = 4;
+    for (int64_t c0 = 0; c0 < count; c0 += Q) {
+        const int64_t nq = std::min(Q, count - c0);
+        if (nodes != nullptr) std::copy(nodes + c0, nodes + c0 + nq, hq.begin());
+        else std::iota(hq.begin(), hq.begin() + nq, (int32_t)c0);
+        CU(cudaMemcpyAsync(dq.p, hq.data(), sizeof(int32_t) * (size_t)nq, cudaMemcpyHostToDevice, ctx->stream));
+        rec_count_kernel<<<(unsigned)((nq + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(ctx->d_rowptr, ctx->d_col, dq.p, nq, dcnt.p);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(hcnt.data(), dcnt.p, sizeof(int64_t) * (size_t)nq, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        // batches: consecutive nodes whose segments fit the bound together; the offsets are the exclusive scan of the counts
+        for (int64_t b0 = 0; b0 < nq;) {
+            int64_t b1 = b0, total = 0;
+            hoff[0] = 0;
+            while (b1 < nq && (b1 == b0 || total + hcnt[(size_t)b1] <= budget_keys)) {
+                total += hcnt[(size_t)b1];
+                hoff[(size_t)(b1 - b0 + 1)] = total;
+                ++b1;
+            }
+            if (keys.reserve((size_t)total) != cudaSuccess) {
+                if (b1 - b0 == 1)
+                    return fail(ctx, BIGCLAM_ENOMEM, "%s: node %d has %lld two-hop entries; no room for their %lld-byte scratch", what,
+                                hq[(size_t)b0], (long long)total, (long long)(total * (int64_t)sizeof(uint32_t)));
+                return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte scratch", what, (long long)(total * (int64_t)sizeof(uint32_t)));
+            }
+            const int64_t nb = b1 - b0;
+            CU(cudaMemcpyAsync(doff.p, hoff.data(), sizeof(int64_t) * (size_t)(nb + 1), cudaMemcpyHostToDevice, ctx->stream));
+            const unsigned grid = (unsigned)((nb + wpb - 1) / wpb);
+            rec_fill_kernel<<<grid, 32 * wpb, 0, ctx->stream>>>(ctx->d_rowptr, ctx->d_col, dq.p + b0, nb, doff.p, keys.p);
+            CU(cudaGetLastError());
+            rec_rank_kernel<<<grid, 32 * wpb, 0, ctx->stream>>>(s, dq.p + b0, nb, doff.p, keys.p, m, dv.p + (size_t)b0 * m,
+                                                               dx.p + (size_t)b0 * m, found_out != nullptr ? dfound.p + b0 : nullptr);
+            CU(cudaGetLastError());
+            CU(cudaStreamSynchronize(ctx->stream));        // (hoff is reused by the next batch)
+            b0 = b1;
+        }
+        CU(cudaMemcpyAsync(v_out + (size_t)c0 * m, dv.p, sizeof(int32_t) * (size_t)nq * m, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(x_out + (size_t)c0 * m, dx.p, sizeof(double) * (size_t)nq * m, cudaMemcpyDeviceToHost, ctx->stream));
+        if (found_out != nullptr)
+            CU(cudaMemcpyAsync(found_out + c0, dfound.p, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    return BIGCLAM_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Fused collective of the node-partitioned path: exchange buffers (see bigclam_ctx::x_*).
 static int xchg_alloc(bigclam_ctx *ctx, int32_t world, int32_t rank) {
     if (world < 1 || world > 8 || rank < 0 || rank >= world) return fail(ctx, BIGCLAM_EINVAL, "exchange buffers: bad world/rank (at most 8 GPUs)");
@@ -1948,6 +2099,19 @@ extern "C" int bigclam_multi_get_F_nnz(bigclam_multi *m, int64_t *nnz_out) {
 extern "C" int bigclam_multi_get_F_csr(bigclam_multi *m, int64_t *indptr_out, int32_t *indices_out, double *values_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     MCALL(bigclam_get_F_csr(m->r[0], indptr_out, indices_out, values_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+
+// Edge probabilities and recommendations read rank 0's replica (all replicas hold the same rows).
+extern "C" int bigclam_multi_pair_affinity(bigclam_multi *m, const int32_t *u, const int32_t *v, int64_t count, double *x_out, double *p_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_pair_affinity(m->r[0], u, v, count, x_out, p_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_recommend(bigclam_multi *m, const int32_t *nodes, int64_t count, int32_t mm, int32_t *v_out, double *x_out,
+                                       int32_t *found_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_recommend(m->r[0], nodes, count, mm, v_out, x_out, found_out), m->r[0]);
     return BIGCLAM_OK;
 }
 

@@ -1039,4 +1039,179 @@ __global__ void sparse_to_dense_kernel(const uint64_t *hdr, const double *pool, 
     for (int i = lane; i < cnt; i += 32) row[idx[i]] = vals[i];
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Edge probabilities and link recommendations from the current F (read only; bigclam_pair_affinity / bigclam_recommend).
+//
+// The affinity x_uv is the sum of F_uc F_vc over the components c that are non-zero in BOTH rows, folded left in
+// ascending c with every product and every sum rounded on its own: the same bits for sparse and dense rows, for (u, v)
+// and (v, u), and for a NumPy restatement.  p_uv = 1 - clamp(exp(-x), MIN_P_, MAX_P_), the clamp of
+// bigclam4-7.scala:166, so log(p_uv) + x_uv is the per-edge term of the LLH (:218).
+struct RowSrc {                    // the rows of the current F: sparse (hdr, pool) when hdr != nullptr, else dense (F, ld)
+    const uint64_t *hdr;
+    const double *pool;
+    const double *F;
+    int32_t k, ld;
+};
+struct PairConst {                 // the clamp of p, with the step kernel's exact shortcuts (fill_args)
+    double min_p, max_p, x_lo, x_hi;
+};
+
+__device__ __forceinline__ double pair_x(const RowSrc &s, int64_t u, int64_t v) {
+    double x = 0.0;
+    if (s.hdr != nullptr) {        // merge of the two ascending index lists
+        const uint64_t hu = s.hdr[u], hv = s.hdr[v];
+        const uint32_t cu = sp_cnt(hu), cv = sp_cnt(hv);
+        const double *au = s.pool + sp_off8(hu), *av = s.pool + sp_off8(hv);
+        const unsigned short *iu = sp_idx(au, cu), *iv = sp_idx(av, cv);
+        uint32_t i = 0, j = 0;
+        while (i < cu && j < cv) {
+            const unsigned short a = iu[i], b = iv[j];
+            if (a == b) { x = __dadd_rn(x, __dmul_rn(au[i], av[j])); ++i; ++j; }
+            else if (a < b) ++i;
+            else ++j;
+        }
+        return x;
+    }
+    const double *fu = s.F + (size_t)u * s.ld, *fv = s.F + (size_t)v * s.ld;
+    for (int c = 0; c < s.k; ++c) {
+        const double a = fu[c], b = fv[c];
+        if (a != 0.0 && b != 0.0) x = __dadd_rn(x, __dmul_rn(a, b));
+    }
+    return x;
+}
+
+__device__ __forceinline__ double pair_p(double x, const PairConst &c) {
+    double e;
+    if (x <= c.x_lo) e = c.max_p;
+    else if (x >= c.x_hi) e = c.min_p;
+    else e = fmin(fmax(exp_neg(x), c.min_p), c.max_p);      // (next to the shortcuts the clamp may still bite)
+    return 1.0 - e;
+}
+
+// One lane per pair.
+__global__ void pair_affinity_kernel(RowSrc s, PairConst pc, const int32_t *__restrict__ u, const int32_t *__restrict__ v,
+                                     int64_t count, double *__restrict__ x_out, double *__restrict__ p_out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const double x = pair_x(s, u[i], v[i]);
+    x_out[i] = x;
+    if (p_out != nullptr) p_out[i] = pair_p(x, pc);
+}
+
+// Recommendations, one warp per query node u of a batch.  The two-hop list of u is, in one segment of a key scratch:
+// 2u and 2w for every w in N(u) (entries that exclude a node), then 2v + 1 for every v in N(w), w in N(u) (candidates).
+// Sorted ascending, the first key of every run of equal v >> 1 tells whether v is excluded: repeated and unsorted
+// neighbour lists need no preparation.
+//   count  entries of u's segment: 1 + deg(u) + sum_{w in N(u)} deg(w)
+__global__ void rec_count_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ col,
+                                 const int32_t *__restrict__ q, int64_t nq, int64_t *__restrict__ cnt) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (i >= nq) return;                                     // (warp-uniform)
+    const int64_t u = q[i], e0 = rowptr[u], e1 = rowptr[u + 1];
+    long long t = 0;
+    for (int64_t e = e0 + lane; e < e1; e += 32) {
+        const int32_t w = col[e];
+        t += rowptr[w + 1] - rowptr[w];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (lane == 0) cnt[i] = 1 + (e1 - e0) + t;
+}
+
+//   fill   the segment at off[i] (offsets relative to the batch's scratch)
+__global__ void rec_fill_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ col,
+                                const int32_t *__restrict__ q, int64_t nq, const int64_t *__restrict__ off,
+                                uint32_t *__restrict__ keys) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (i >= nq) return;
+    const int64_t u = q[i], e0 = rowptr[u], e1 = rowptr[u + 1];
+    uint32_t *seg = keys + off[i];
+    if (lane == 0) seg[0] = 2u * (uint32_t)u;
+    for (int64_t e = e0 + lane; e < e1; e += 32) seg[1 + (e - e0)] = 2u * (uint32_t)col[e];
+    int64_t pos = 1 + (e1 - e0);
+    for (int64_t e = e0; e < e1; ++e) {
+        const int32_t w = col[e];
+        const int64_t f0 = rowptr[w], f1 = rowptr[w + 1];
+        for (int64_t f = f0 + lane; f < f1; f += 32) seg[pos + (f - f0)] = 2u * (uint32_t)col[f] + 1u;
+        pos += f1 - f0;
+    }
+}
+
+// (x, v) ranks before (y, w): larger affinity first, then the smaller node id
+__device__ __forceinline__ bool rec_better(double x, int32_t v, double y, int32_t w) { return x > y || (x == y && v < w); }
+
+//   rank   sort the segment (a bitonic network whose comparators all put the smaller key first, so the keys beyond the
+//          segment's end act as +inf and never move), then score every candidate that survives (pair_x) and keep the m
+//          best with x > 0 in v_out / x_out (rows of m, padded with -1 / 0); found = how many were kept
+__global__ void rec_rank_kernel(RowSrc s, const int32_t *__restrict__ q, int64_t nq, const int64_t *__restrict__ off,
+                                uint32_t *__restrict__ keys, int32_t m, int32_t *__restrict__ v_out, double *__restrict__ x_out,
+                                int32_t *__restrict__ found) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (i >= nq) return;
+    const int64_t u = q[i];
+    uint32_t *seg = keys + off[i];
+    const int64_t L = off[i + 1] - off[i];
+    int lgp = 0;
+    while (((int64_t)1 << lgp) < L) ++lgp;
+    const int64_t npairs = ((int64_t)1 << lgp) >> 1;
+    for (int lg = 1; lg <= lgp; ++lg) {
+        const int64_t size = (int64_t)1 << lg, hmask = (size >> 1) - 1;
+        for (int64_t t = lane; t < npairs; t += 32) {             // the flip: j <-> size - 1 - j inside a block of size
+            const int64_t base = (t >> (lg - 1)) << lg, j = t & hmask;
+            const int64_t lo = base + j, hi = base + size - 1 - j;
+            if (hi < L) {
+                const uint32_t a = seg[lo], c = seg[hi];
+                if (a > c) { seg[lo] = c; seg[hi] = a; }
+            }
+        }
+        __syncwarp();
+        for (int ls = lg - 2; ls >= 0; --ls) {                    // half-cleaners: j <-> j + stride
+            const int64_t stride = (int64_t)1 << ls;
+            for (int64_t t = lane; t < npairs; t += 32) {
+                const int64_t lo = ((t >> ls) << (ls + 1)) + (t & (stride - 1)), hi = lo + stride;
+                if (hi < L) {
+                    const uint32_t a = seg[lo], c = seg[hi];
+                    if (a > c) { seg[lo] = c; seg[hi] = a; }
+                }
+            }
+            __syncwarp();
+        }
+    }
+    int32_t *vo = v_out + (size_t)i * m;
+    double *xo = x_out + (size_t)i * m;
+    for (int t = lane; t < m; t += 32) { vo[t] = -1; xo[t] = 0.0; }
+    __syncwarp();
+    int kept = 0;                                            // (warp-uniform)
+    double xw = 0.0;                                         // the last kept entry, once the list is full
+    int32_t vw = 0;
+    for (int64_t t0 = 0; t0 < L; t0 += 32) {
+        const int64_t t = t0 + lane;
+        const uint32_t key = (t < L) ? seg[t] : 0u;
+        const bool cand = (t < L) && (key & 1u) && (t == 0 || (seg[t - 1] >> 1) != (key >> 1));
+        const int32_t v = (int32_t)(key >> 1);
+        const double x = cand ? pair_x(s, u, v) : 0.0;
+        unsigned want = __ballot_sync(0xffffffffu, cand && x > 0.0 && (kept < m || rec_better(x, v, xw, vw)));
+        while (want) {                                       // insertions in lane order, by lane 0
+            const int l = __ffs(want) - 1;
+            want &= want - 1u;
+            const double xb = __shfl_sync(0xffffffffu, x, l);
+            const int32_t vb = __shfl_sync(0xffffffffu, v, l);
+            if (lane == 0 && (kept < m || rec_better(xb, vb, xo[m - 1], vo[m - 1]))) {
+                int p = (kept < m) ? kept : m - 1;
+                while (p > 0 && rec_better(xb, vb, xo[p - 1], vo[p - 1])) { xo[p] = xo[p - 1]; vo[p] = vo[p - 1]; --p; }
+                xo[p] = xb;
+                vo[p] = vb;
+                if (kept < m) ++kept;
+            }
+            kept = __shfl_sync(0xffffffffu, kept, 0);
+        }
+        __syncwarp();
+        if (kept == m) { xw = xo[m - 1]; vw = vo[m - 1]; }
+    }
+    if (lane == 0 && found != nullptr) found[i] = kept;
+}
+
 }  // namespace bigclam

@@ -359,6 +359,41 @@ class BigClam:
             LLHKold = LLHKnew
         return KforC, hist
 
+    # ---- the fitted model as a model of edges: P(u,v) = 1 - exp(-F_u.F_v), clamped like :166 ----
+    def edge_probability(self, u, v):
+        """Affinity x = F_u.F_v and edge probability p = 1 - clamp(exp(-x), MIN_P_, MAX_P_) of the pairs (u[i], v[i]),
+        computed on the GPU from the current F.  Returns (x, p) float64 arrays."""
+        u = np.ascontiguousarray(u, dtype=np.int32).ravel()
+        v = np.ascontiguousarray(v, dtype=np.int32).ravel()
+        if len(u) != len(v):
+            raise ValueError("u and v must have the same length")
+        x = np.empty(len(u), dtype=np.float64)
+        p = np.empty(len(u), dtype=np.float64)
+        if self._multi is not None:
+            self._mcheck(_lib.load().bigclam_multi_pair_affinity(self._multi, u.ctypes.data, v.ctypes.data, len(u),
+                                                                 x.ctypes.data, p.ctypes.data))
+        else:
+            check(_lib.load().bigclam_pair_affinity(self._need(), u.ctypes.data, v.ctypes.data, len(u), x.ctypes.data,
+                                                    p.ctypes.data), self._ctx)
+        return x, p
+
+    def recommend(self, nodes=None, m: int = 10):
+        """For each query node u (None = all nodes), the m not-yet-linked nodes at distance 2 with the largest affinity
+        x > 0, by x descending then id ascending.  Returns (v, x) arrays of shape len(nodes) x m, padded with -1 and 0."""
+        cnt = self.n if nodes is None else None
+        ptr = None
+        if nodes is not None:
+            nodes = np.ascontiguousarray(nodes, dtype=np.int32).ravel()
+            cnt, ptr = len(nodes), nodes.ctypes.data
+        m = int(m)
+        vo = np.empty((cnt, max(m, 0)), dtype=np.int32)
+        xo = np.empty((cnt, max(m, 0)), dtype=np.float64)
+        if self._multi is not None:
+            self._mcheck(_lib.load().bigclam_multi_recommend(self._multi, ptr, cnt, m, vo.ctypes.data, xo.ctypes.data, None))
+        else:
+            check(_lib.load().bigclam_recommend(self._need(), ptr, cnt, m, vo.ctypes.data, xo.ctypes.data, None), self._ctx)
+        return vo, xo
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

@@ -278,6 +278,37 @@ void bigclam_graph_free(bigclam_graph *g);
 int bigclam_extract(bigclam_ctx *ctx, double delta, uint8_t *member_out, double *fmax_out);
 
 /*
+ * The fitted model as a model of edges (the clamp of bigclam4-7.scala:166, the edge term of :218), on the current F:
+ *   x_uv = sum of F_uc * F_vc over the components c that are non-zero in both rows, folded left in ascending c with
+ *          every product and every sum rounded on its own (the same bits for sparse and dense rows and for (v, u));
+ *   p_uv = 1 - clamp(exp(-x_uv), min_p, max_p), so log(p_uv) + x_uv is the per-edge term of the LLH.
+ * Both calls read F only: no state changes (F, sumF, accepted indices, a speculative step of bigclam_step), no dense
+ * n x k image; they run on the context's stream and are synchronous.  Host buffers in and out; ids outside [0, n),
+ * count < 0, m < 1 or a NULL required buffer give BIGCLAM_EINVAL before any device work.  count == 0 is a no-op.
+ *
+ * bigclam_pair_affinity: x_out[i] = x(u[i], v[i]); p_out (optional) the p of the same pairs.  Any count (the pairs are
+ * moved in bounded chunks).
+ */
+int bigclam_pair_affinity(bigclam_ctx *ctx, const int32_t *u, const int32_t *v, int64_t count,
+                          double *x_out, double *p_out /* optional */);
+/*
+ * bigclam_recommend: for each query node u (nodes NULL = all n nodes in id order, then count must be n), the m nodes v
+ * at distance 2 (a neighbour of a neighbour, not u and not in N(u); repeated or unsorted neighbour lists are fine) with
+ * the largest x_uv > 0, by x descending, then v ascending.  A pair with x = 0 has the floor probability 1 - max_p and is
+ * never returned.  v_out / x_out: count x m, row i padded with -1 / 0 after its found_out[i] (optional) entries.  Two-hop
+ * lists are built in batches whose scratch stays within the smaller of 1 GiB and 10 % of the free device memory; a node
+ * whose list alone is longer gets scratch of its own, and BIGCLAM_ENOMEM (naming the node) only when that fails.
+ */
+int bigclam_recommend(bigclam_ctx *ctx, const int32_t *nodes /* NULL = all n */, int64_t count, int32_t m,
+                      int32_t *v_out /* count x m, -1 padded */, double *x_out /* count x m, 0 padded */,
+                      int32_t *found_out /* count, optional */);
+/* The same for a multi-GPU handle: rank 0's replica is read, errors go to bigclam_multi_last_error. */
+int bigclam_multi_pair_affinity(bigclam_multi *m, const int32_t *u, const int32_t *v, int64_t count,
+                                double *x_out, double *p_out);
+int bigclam_multi_recommend(bigclam_multi *m, const int32_t *nodes, int64_t count, int32_t mm,
+                            int32_t *v_out, double *x_out, int32_t *found_out);
+
+/*
  * Callers in front of the hot path (host side, one-off integer graph work; SURVEY.md §8f-2).
  * bigclam_conductance_seeds = conductanceLocalMin() (bigclam4-7.scala:58-73): ego-net conductance of every
  * node, candidates = the min-id neighbour of each node (tuple .min at :70), ranked by conductance ascending

@@ -16,6 +16,7 @@
 //   MBSGD()       bigclamv3-7.scala:206-222, Bigclamv2.scala:203-219   MBSGD(version)
 //   K sweep                                           :244-266   sweep_K()
 //   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta)
+//   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m)
 //
 // Errors: the reference throws JVM exceptions; here every negative return code of the C ABI becomes a bigclam::Error
 // (std::runtime_error carrying the code and bigclam_last_error()).  There is no CPU path: without a CUDA device
@@ -213,6 +214,31 @@ public:
             for (int c = 0; c < K_; ++c)
                 if (member[(size_t)(u * K_ + c)]) comms[(size_t)c].push_back((int32_t)u);
         return comms;
+    }
+
+    // The fitted model as a model of edges, P(u,v) = 1 - exp(-F_u.F_v) with the clamp of :166 (bigclam_pair_affinity):
+    // x[i] = F_u[i].F_v[i] and p[i] = 1 - clamp(exp(-x[i]), MIN_P_, MAX_P_).  Works for multi-GPU handles too.
+    void edge_probability(const std::vector<int32_t> &u, const std::vector<int32_t> &v, std::vector<double> &x, std::vector<double> &p) {
+        need();
+        if (u.size() != v.size()) throw Error(BIGCLAM_EINVAL, "edge_probability: u and v differ in length");
+        x.assign(u.size(), 0.0);
+        p.assign(u.size(), 0.0);
+        const int64_t cnt = (int64_t)u.size();
+        check(multi_ ? bigclam_multi_pair_affinity(multi_, u.data(), v.data(), cnt, x.data(), p.data())
+                     : bigclam_pair_affinity(ctx_, u.data(), v.data(), cnt, x.data(), p.data()),
+              "edge_probability");
+    }
+    // For each query node (empty = all nodes) the m nodes at distance 2, not yet linked, with the largest affinity x > 0
+    // (x descending, then id ascending): v and x are nodes.size() x m row-major, padded with -1 and 0 (bigclam_recommend).
+    void recommend(const std::vector<int32_t> &nodes, int m, std::vector<int32_t> &v, std::vector<double> &x) {
+        need();
+        const int64_t cnt = nodes.empty() ? n_ : (int64_t)nodes.size();
+        const int32_t *q = nodes.empty() ? nullptr : nodes.data();
+        v.assign((size_t)(cnt * std::max(m, 0)), -1);
+        x.assign((size_t)(cnt * std::max(m, 0)), 0.0);
+        check(multi_ ? bigclam_multi_recommend(multi_, q, cnt, m, v.data(), x.data(), nullptr)
+                     : bigclam_recommend(ctx_, q, cnt, m, v.data(), x.data(), nullptr),
+              "recommend");
     }
 
     std::vector<int> Kset() const { return bigclam::Kset(minCom, maxCom, divCom); }
