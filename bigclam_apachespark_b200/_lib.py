@@ -122,6 +122,10 @@ SIGNATURES = {
     "bigclam_recommend": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "bigclam_multi_pair_affinity": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp]),
     "bigclam_multi_recommend": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "bigclam_sample_graph_nnz": (C.c_int, [_vp, C.c_uint64, _dbl, _pi64]),
+    "bigclam_sample_graph": (C.c_int, [_vp, C.c_uint64, _dbl, _vp, _vp]),
+    "bigclam_multi_sample_graph_nnz": (C.c_int, [_vp, C.c_uint64, _dbl, _pi64]),
+    "bigclam_multi_sample_graph": (C.c_int, [_vp, C.c_uint64, _dbl, _vp, _vp]),
     "bigclam_conductance_seeds": (C.c_int, [_i64, _vp, _vp, _vp, _vp, _pi64]),
     "bigclam_conductance_seeds_gpu": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _vp, _pi64]),
     "bigclam_init_neighbor_com_F": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _i64, _i32, C.c_uint64, _vp]),

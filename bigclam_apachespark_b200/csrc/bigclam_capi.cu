@@ -1757,6 +1757,10 @@ static RowSrc row_src(const bigclam_ctx *ctx) {
     return s;
 }
 
+static PairConst pair_const(const bigclam_ctx *ctx) {
+    return PairConst{ctx->p.min_p, ctx->p.max_p, -std::log(ctx->p.max_p) * (1.0 - 1e-12), -std::log(ctx->p.min_p) * (1.0 + 1e-12)};
+}
+
 static int check_ids(bigclam_ctx *ctx, const char *what, const char *name, const int32_t *ids, int64_t count) {
     for (int64_t i = 0; i < count; ++i)
         if (ids[i] < 0 || ids[i] >= ctx->n)
@@ -1774,7 +1778,7 @@ extern "C" int bigclam_pair_affinity(bigclam_ctx *ctx, const int32_t *u, const i
     if (int rc = check_ids(ctx, what, "v", v, count)) return rc;
     CU(cudaSetDevice(ctx->device));
     const RowSrc s = row_src(ctx);
-    const PairConst pc{ctx->p.min_p, ctx->p.max_p, -std::log(ctx->p.max_p) * (1.0 - 1e-12), -std::log(ctx->p.min_p) * (1.0 + 1e-12)};
+    const PairConst pc = pair_const(ctx);
     const int64_t chunk = std::min<int64_t>(count, (int64_t)1 << 22);      // pairs per transfer
     DevBuf<int32_t> du, dv;
     DevBuf<double> dx, dp;
@@ -1868,6 +1872,112 @@ extern "C" int bigclam_recommend(bigclam_ctx *ctx, const int32_t *nodes, int64_t
         if (found_out != nullptr)
             CU(cudaMemcpyAsync(found_out + c0, dfound.p, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
+    }
+    return BIGCLAM_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// A graph sampled from the model (bigclam_sparse.cuh, sample_rows_kernel): the column index of the current rows, every
+// row's degree, then the rows in batches.  Reads F only, on the context's stream, like the calls above.
+struct SamplePlan {
+    DevBuf<int64_t> colptr;
+    DevBuf<int32_t> members;
+    SampleArgs a{};
+};
+
+static int sample_args_check(bigclam_ctx *ctx, const char *what, double eps, const void *out1, const void *out2) {
+    if (!(eps >= 0.0 && eps < 1.0)) return fail(ctx, BIGCLAM_EINVAL, "%s: eps = %g, must be in [0, 1)", what, eps);
+    if (out1 == nullptr || out2 == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: NULL output", what);
+    return BIGCLAM_OK;
+}
+
+// Builds the column index into pl and writes the sampled degrees' exclusive scan to rowptr (host, n + 1 entries).
+static int sample_count(bigclam_ctx *ctx, uint64_t seed, double eps, SamplePlan &pl, int64_t *rowptr) {
+    CU(cudaSetDevice(ctx->device));
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k;
+    const int wpb = 4;
+    const RowSrc s = row_src(ctx);
+    rowptr[0] = 0;
+    if (n == 0) return BIGCLAM_OK;
+    const unsigned grid_n = (unsigned)((n + wpb - 1) / wpb);
+    DevBuf<unsigned int> ccnt;
+    DevBuf<unsigned long long> cpos;
+    DevBuf<int64_t> deg;
+    CU(ccnt.reserve((size_t)k));
+    CU(cudaMemsetAsync(ccnt.p, 0, sizeof(unsigned int) * (size_t)k, ctx->stream));
+    colidx_kernel<false><<<grid_n, 32 * wpb, 0, ctx->stream>>>(s, n, ccnt.p, nullptr, nullptr);
+    CU(cudaGetLastError());
+    std::vector<unsigned int> hcnt((size_t)k);
+    CU(cudaMemcpyAsync(hcnt.data(), ccnt.p, sizeof(unsigned int) * (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    std::vector<int64_t> hptr((size_t)k + 1, 0);
+    for (int32_t c = 0; c < k; ++c) hptr[(size_t)c + 1] = hptr[(size_t)c] + hcnt[(size_t)c];
+    std::vector<unsigned long long> hpos(hptr.begin(), hptr.end() - 1);
+    CU(pl.colptr.reserve((size_t)k + 1));
+    CU(pl.members.reserve((size_t)hptr[(size_t)k]));
+    CU(cpos.reserve((size_t)k));
+    CU(cudaMemcpyAsync(pl.colptr.p, hptr.data(), sizeof(int64_t) * ((size_t)k + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(cpos.p, hpos.data(), sizeof(unsigned long long) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
+    colidx_kernel<true><<<grid_n, 32 * wpb, 0, ctx->stream>>>(s, n, nullptr, cpos.p, pl.members.p);
+    CU(cudaGetLastError());
+    colidx_sort_kernel<<<(unsigned)((k + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(pl.colptr.p, k, pl.members.p);
+    CU(cudaGetLastError());
+    pl.a = SampleArgs{s, pair_const(ctx), pl.colptr.p, pl.members.p, n, seed, eps};
+    CU(deg.reserve((size_t)n));
+    sample_rows_kernel<false><<<grid_n, 32 * wpb, 0, ctx->stream>>>(pl.a, 0, n, deg.p, nullptr, 0, nullptr);
+    CU(cudaGetLastError());
+    std::vector<int64_t> hdeg((size_t)n);
+    CU(cudaMemcpyAsync(hdeg.data(), deg.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (int64_t u = 0; u < n; ++u) rowptr[u + 1] = rowptr[u] + hdeg[(size_t)u];
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_sample_graph_nnz(bigclam_ctx *ctx, uint64_t seed, double eps, int64_t *nnz_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    if (int rc = sample_args_check(ctx, "bigclam_sample_graph_nnz", eps, nnz_out, nnz_out)) return rc;
+    SamplePlan pl;
+    std::vector<int64_t> rowptr((size_t)ctx->n + 1);
+    if (int rc = sample_count(ctx, seed, eps, pl, rowptr.data())) return rc;
+    *nnz_out = rowptr[(size_t)ctx->n];
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_sample_graph(bigclam_ctx *ctx, uint64_t seed, double eps, int64_t *rowptr_out, int32_t *col_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_sample_graph";
+    if (int rc = sample_args_check(ctx, what, eps, rowptr_out, col_out)) return rc;
+    SamplePlan pl;
+    if (int rc = sample_count(ctx, seed, eps, pl, rowptr_out)) return rc;
+    const int64_t n = ctx->n;
+    if (rowptr_out[n] == 0) return BIGCLAM_OK;
+    // batches of consecutive rows whose output stays within the smaller of 1 GiB and 10 % of the free memory; a row
+    // longer than that alone gets a batch of its own
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    const int64_t budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    const int64_t budget_entries = std::max<int64_t>(1, budget / (int64_t)sizeof(int32_t));
+    DevBuf<int64_t> drowptr;
+    DevBuf<int32_t> dout;
+    CU(drowptr.reserve((size_t)n + 1));
+    CU(cudaMemcpyAsync(drowptr.p, rowptr_out, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    const int wpb = 4;
+    for (int64_t b0 = 0; b0 < n;) {
+        int64_t b1 = b0 + 1;
+        while (b1 < n && rowptr_out[b1 + 1] - rowptr_out[b0] <= budget_entries) ++b1;
+        const int64_t total = rowptr_out[b1] - rowptr_out[b0];
+        if (total > 0) {
+            if (dout.reserve((size_t)total) != cudaSuccess)
+                return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte batch of rows %lld..%lld", what,
+                            (long long)(total * (int64_t)sizeof(int32_t)), (long long)b0, (long long)(b1 - 1));
+            sample_rows_kernel<true><<<(unsigned)((b1 - b0 + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(pl.a, b0, b1, nullptr, drowptr.p,
+                                                                                                         rowptr_out[b0], dout.p);
+            CU(cudaGetLastError());
+            CU(cudaMemcpyAsync(col_out + rowptr_out[b0], dout.p, sizeof(int32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaStreamSynchronize(ctx->stream));
+        }
+        b0 = b1;
     }
     return BIGCLAM_OK;
 }
@@ -2112,6 +2222,16 @@ extern "C" int bigclam_multi_recommend(bigclam_multi *m, const int32_t *nodes, i
                                        int32_t *found_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     MCALL(bigclam_recommend(m->r[0], nodes, count, mm, v_out, x_out, found_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_sample_graph_nnz(bigclam_multi *m, uint64_t seed, double eps, int64_t *nnz_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_sample_graph_nnz(m->r[0], seed, eps, nnz_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_sample_graph(bigclam_multi *m, uint64_t seed, double eps, int64_t *rowptr_out, int32_t *col_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_sample_graph(m->r[0], seed, eps, rowptr_out, col_out), m->r[0]);
     return BIGCLAM_OK;
 }
 

@@ -1142,18 +1142,9 @@ __global__ void rec_fill_kernel(const int64_t *__restrict__ rowptr, const int32_
 // (x, v) ranks before (y, w): larger affinity first, then the smaller node id
 __device__ __forceinline__ bool rec_better(double x, int32_t v, double y, int32_t w) { return x > y || (x == y && v < w); }
 
-//   rank   sort the segment (a bitonic network whose comparators all put the smaller key first, so the keys beyond the
-//          segment's end act as +inf and never move), then score every candidate that survives (pair_x) and keep the m
-//          best with x > 0 in v_out / x_out (rows of m, padded with -1 / 0); found = how many were kept
-__global__ void rec_rank_kernel(RowSrc s, const int32_t *__restrict__ q, int64_t nq, const int64_t *__restrict__ off,
-                                uint32_t *__restrict__ keys, int32_t m, int32_t *__restrict__ v_out, double *__restrict__ x_out,
-                                int32_t *__restrict__ found) {
-    const int lane = threadIdx.x & 31;
-    const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (i >= nq) return;
-    const int64_t u = q[i];
-    uint32_t *seg = keys + off[i];
-    const int64_t L = off[i + 1] - off[i];
+// Sorts seg[0, L) ascending in place, by the whole warp: a bitonic network whose comparators all put the smaller key
+// first, so the keys beyond the segment's end act as +inf and never move.  Ends with the warp in step.
+__device__ __forceinline__ void warp_sort_u32(uint32_t *seg, int64_t L, int lane) {
     int lgp = 0;
     while (((int64_t)1 << lgp) < L) ++lgp;
     const int64_t npairs = ((int64_t)1 << lgp) >> 1;
@@ -1180,6 +1171,20 @@ __global__ void rec_rank_kernel(RowSrc s, const int32_t *__restrict__ q, int64_t
             __syncwarp();
         }
     }
+}
+
+//   rank   sort the segment (warp_sort_u32), then score every candidate that survives (pair_x) and keep the m best with
+//          x > 0 in v_out / x_out (rows of m, padded with -1 / 0); found = how many were kept
+__global__ void rec_rank_kernel(RowSrc s, const int32_t *__restrict__ q, int64_t nq, const int64_t *__restrict__ off,
+                                uint32_t *__restrict__ keys, int32_t m, int32_t *__restrict__ v_out, double *__restrict__ x_out,
+                                int32_t *__restrict__ found) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (i >= nq) return;
+    const int64_t u = q[i];
+    uint32_t *seg = keys + off[i];
+    const int64_t L = off[i + 1] - off[i];
+    warp_sort_u32(seg, L, lane);
     int32_t *vo = v_out + (size_t)i * m;
     double *xo = x_out + (size_t)i * m;
     for (int t = lane; t < m; t += 32) { vo[t] = -1; xo[t] = 0.0; }
@@ -1212,6 +1217,164 @@ __global__ void rec_rank_kernel(RowSrc s, const int32_t *__restrict__ q, int64_t
         if (kept == m) { xw = xo[m - 1]; vw = vo[m - 1]; }
     }
     if (lane == 0 && found != nullptr) found[i] = kept;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// A graph sampled from the model (read only; bigclam_sample_graph).  For every unordered pair u < v of the n nodes:
+//   shared      rows u and v have a component that is non-zero in both: p_uv = pair_p(pair_x(u, v)), the bits of
+//               bigclam_pair_affinity's p (its floor 1 - MAX_P_ included);
+//   not shared  p_uv = eps, the caller's background probability (0 <= eps < 1);
+// and the pair is an edge iff r(seed, u, v) < p_uv, with
+//   key = (uint64)u << 32 | v,  h = mix(seed ^ mix(key)),  r = (h >> 11) * 2^-53,
+// mix = the splitmix64 step.  The result is a function of (F bits, seed, eps, min_p, max_p) only.
+//
+// Row u decides all of its pairs, v < u and v > u, so every pair is decided twice, once from each end, with the same
+// bits (x, p and r are symmetric): no transpose and no symmetrisation, and any cut of the rows into batches works.
+//   co-member pairs  for c in supp(u), v in M_c (the column index below), v != u: one merge of the two rows gives x_uv
+//                    and the first shared component; the pair is taken at that component only, so once per row;
+//   background       (eps > 0) lanes stride over all v != u and hash first; only a hit (an eps fraction) pays the merge
+//                    that checks the two rows share nothing.
+// count gives the row's degree; fill writes the row at its offset, then sorts it (warp_sort_u32).
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+__host__ __device__ __forceinline__ double sample_r(uint64_t seed, int64_t u, int64_t v) {
+    const uint64_t lo = (uint64_t)(u < v ? u : v), hi = (uint64_t)(u < v ? v : u);
+    const uint64_t h = splitmix64(seed ^ splitmix64(lo << 32 | hi));
+    return (double)(h >> 11) * 0x1.0p-53;
+}
+
+// pair_x's fold (the same bits) and the first component that is non-zero in both rows (-1: none)
+__device__ __forceinline__ double pair_x_first(const RowSrc &s, int64_t u, int64_t v, int &first) {
+    double x = 0.0;
+    first = -1;
+    if (s.hdr != nullptr) {
+        const uint64_t hu = s.hdr[u], hv = s.hdr[v];
+        const uint32_t cu = sp_cnt(hu), cv = sp_cnt(hv);
+        const double *au = s.pool + sp_off8(hu), *av = s.pool + sp_off8(hv);
+        const unsigned short *iu = sp_idx(au, cu), *iv = sp_idx(av, cv);
+        uint32_t i = 0, j = 0;
+        while (i < cu && j < cv) {
+            const unsigned short a = iu[i], b = iv[j];
+            if (a == b) {
+                if (first < 0 && au[i] != 0.0 && av[j] != 0.0) first = a;
+                x = __dadd_rn(x, __dmul_rn(au[i], av[j]));
+                ++i;
+                ++j;
+            } else if (a < b) ++i;
+            else ++j;
+        }
+        return x;
+    }
+    const double *fu = s.F + (size_t)u * s.ld, *fv = s.F + (size_t)v * s.ld;
+    for (int c = 0; c < s.k; ++c) {
+        const double a = fu[c], b = fv[c];
+        if (a != 0.0 && b != 0.0) {
+            if (first < 0) first = c;
+            x = __dadd_rn(x, __dmul_rn(a, b));
+        }
+    }
+    return x;
+}
+
+// Column index of the current rows: colptr[k + 1] and members, M_c = members[colptr[c], colptr[c + 1]) ascending.
+// Built by count, scan (host) and fill, one warp per row; the fill takes slots in any order and the sort makes the
+// lists ascending, so the index is the same from run to run.
+template <bool kFill>
+__global__ void colidx_kernel(RowSrc s, int64_t n, unsigned int *__restrict__ colcnt, unsigned long long *__restrict__ colpos,
+                              int32_t *__restrict__ members) {
+    const int lane = threadIdx.x & 31;
+    const int64_t u = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (u >= n) return;
+    const bool sparse = s.hdr != nullptr;
+    const uint64_t hu = sparse ? s.hdr[u] : 0;
+    const int cnt = sparse ? (int)sp_cnt(hu) : s.k;
+    const double *vals = sparse ? s.pool + sp_off8(hu) : s.F + (size_t)u * s.ld;
+    const unsigned short *idx = sparse ? sp_idx(vals, (uint32_t)cnt) : nullptr;
+    for (int i = lane; i < cnt; i += 32) {
+        if (vals[i] == 0.0) continue;
+        const int c = sparse ? (int)idx[i] : i;
+        if (kFill) members[atomicAdd(&colpos[c], 1ull)] = (int32_t)u;
+        else atomicAdd(&colcnt[c], 1u);
+    }
+}
+
+__global__ void colidx_sort_kernel(const int64_t *__restrict__ colptr, int32_t k, int32_t *__restrict__ members) {
+    const int lane = threadIdx.x & 31;
+    const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (c >= k) return;
+    warp_sort_u32(reinterpret_cast<uint32_t *>(members + colptr[c]), colptr[c + 1] - colptr[c], lane);
+}
+
+struct SampleArgs {
+    RowSrc s;
+    PairConst pc;
+    const int64_t *colptr;             // the column index (colidx_kernel)
+    const int32_t *members;
+    int64_t n;
+    uint64_t seed;
+    double eps;
+};
+
+// One warp per row u of [r0, r1).  count: deg[u - r0] = the row's degree.  fill: the row goes to out[rowptr[u] - base ..),
+// ascending.
+template <bool kFill>
+__global__ void sample_rows_kernel(SampleArgs a, int64_t r0, int64_t r1, int64_t *__restrict__ deg, const int64_t *__restrict__ rowptr,
+                                   int64_t base, int32_t *__restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const int64_t u = r0 + (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (u >= r1) return;                                     // (warp-uniform)
+    const unsigned lt_mask = (1u << lane) - 1u;
+    int32_t *seg = kFill ? out + (rowptr[u] - base) : nullptr;
+    int64_t taken = 0;                                       // (warp-uniform)
+    auto emit = [&](bool take, int64_t v) {
+        const unsigned bal = __ballot_sync(0xffffffffu, take);
+        if (kFill && take) seg[taken + __popc(bal & lt_mask)] = (int32_t)v;
+        taken += __popc(bal);
+    };
+    const RowSrc &s = a.s;
+    const bool sparse = s.hdr != nullptr;
+    const uint64_t hu = sparse ? s.hdr[u] : 0;
+    const int cnt = sparse ? (int)sp_cnt(hu) : s.k;
+    const double *vals = sparse ? s.pool + sp_off8(hu) : s.F + (size_t)u * s.ld;
+    const unsigned short *idx = sparse ? sp_idx(vals, (uint32_t)cnt) : nullptr;
+    for (int i = 0; i < cnt; ++i) {                          // co-member pairs, component by component
+        if (vals[i] == 0.0) continue;
+        const int c = sparse ? (int)idx[i] : i;
+        const int64_t m0 = a.colptr[c], m1 = a.colptr[c + 1];
+        for (int64_t t0 = m0; t0 < m1; t0 += 32) {
+            const int64_t t = t0 + lane;
+            const int64_t v = (t < m1) ? a.members[t] : u;
+            bool take = false;
+            if (v != u) {
+                int first;
+                const double x = pair_x_first(s, u, v, first);
+                take = first == c && sample_r(a.seed, u, v) < pair_p(x, a.pc);
+            }
+            emit(take, v);
+        }
+    }
+    if (a.eps > 0.0) {                                       // background pairs
+        for (int64_t v0 = 0; v0 < a.n; v0 += 32) {
+            const int64_t v = v0 + lane;
+            bool take = false;
+            if (v < a.n && v != u && sample_r(a.seed, u, v) < a.eps) {
+                int first;
+                (void)pair_x_first(s, u, v, first);
+                take = first < 0;
+            }
+            emit(take, v);
+        }
+    }
+    if (!kFill) {
+        if (lane == 0) deg[u - r0] = taken;
+        return;
+    }
+    __syncwarp();
+    warp_sort_u32(reinterpret_cast<uint32_t *>(seg), taken, lane);
 }
 
 }  // namespace bigclam

@@ -394,6 +394,26 @@ class BigClam:
             check(_lib.load().bigclam_recommend(self._need(), ptr, cnt, m, vo.ctypes.data, xo.ctypes.data, None), self._ctx)
         return vo, xo
 
+    def sample_graph(self, seed, eps=0.0):
+        """A graph drawn from the model on the GPU: a pair that shares a component is an edge with probability p_uv (the
+        p of edge_probability), any other pair with probability eps (0 <= eps < 1; 1 - MAX_P_ is the model as coded).
+        The same (F, seed, eps) gives the same graph.  Returns (rowptr int64[n + 1], col int32[nnz]): symmetric, rows
+        ascending, no self loops, the shape set_graph takes."""
+        lib = _lib.load()
+        seed, eps = int(seed) & 0xFFFFFFFFFFFFFFFF, float(eps)
+        nnz = C.c_int64()
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_sample_graph_nnz(self._multi, seed, eps, C.byref(nnz)))
+        else:
+            check(lib.bigclam_sample_graph_nnz(self._need(), seed, eps, C.byref(nnz)), self._ctx)
+        rowptr = np.empty(self.n + 1, dtype=np.int64)
+        col = np.empty(max(nnz.value, 1), dtype=np.int32)
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_sample_graph(self._multi, seed, eps, rowptr.ctypes.data, col.ctypes.data))
+        else:
+            check(lib.bigclam_sample_graph(self._ctx, seed, eps, rowptr.ctypes.data, col.ctypes.data), self._ctx)
+        return rowptr, col[:nnz.value]
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

@@ -309,6 +309,33 @@ int bigclam_multi_recommend(bigclam_multi *m, const int32_t *nodes, int64_t coun
                             int32_t *v_out, double *x_out, int32_t *found_out);
 
 /*
+ * A graph sampled from the model, on the current F.  For every unordered pair u < v of the n nodes:
+ *   shared      rows u and v have at least one component that is non-zero in both: p_uv = the p of
+ *               bigclam_pair_affinity (the same bits, its floor 1 - max_p included);
+ *   not shared  p_uv = eps, a background probability, 0 <= eps < 1: 1 - max_p gives the model as coded (the clamp of
+ *               bigclam4-7.scala:166 applied to every pair), 0 gives community edges only;
+ * and the pair is an edge iff r(seed, u, v) < p_uv, where
+ *   key = (uint64_t)u << 32 | v,   h = mix(seed ^ mix(key)),   r = (h >> 11) * 2^-53,
+ *   mix(z) = the splitmix64 step: z += 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ *            z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)   (all mod 2^64).
+ * The result is a function of (F, seed, eps, min_p, max_p) only: not of the row layout (sparse or dense), the batch
+ * cut, the number of GPUs or the device.  It is a symmetric CSR, the shape bigclam_create takes: rowptr_out (n + 1) and
+ * col_out (nnz), every row ascending, no self loops, no duplicates.
+ *
+ * bigclam_sample_graph_nnz gives nnz; bigclam_sample_graph fills rowptr_out and col_out (sized with the nnz of the
+ * same F, seed and eps; it counts again, nothing is kept between the calls).  Both read F only, like the calls above:
+ * no state changes, no dense n x k image, the context's stream, synchronous.  eps NaN, negative or >= 1, or a NULL
+ * output (col_out included, also for nnz = 0) gives BIGCLAM_EINVAL before any device work.  The rows are decided in
+ * batches whose output stays within the smaller of 1 GiB and 10 % of the free device memory (a longer row gets a batch
+ * of its own); BIGCLAM_ENOMEM when a batch's buffer cannot be allocated.
+ */
+int bigclam_sample_graph_nnz(bigclam_ctx *ctx, uint64_t seed, double eps, int64_t *nnz_out);
+int bigclam_sample_graph(bigclam_ctx *ctx, uint64_t seed, double eps, int64_t *rowptr_out /* n + 1 */, int32_t *col_out /* nnz */);
+/* The same for a multi-GPU handle: rank 0's replica is read, errors go to bigclam_multi_last_error. */
+int bigclam_multi_sample_graph_nnz(bigclam_multi *m, uint64_t seed, double eps, int64_t *nnz_out);
+int bigclam_multi_sample_graph(bigclam_multi *m, uint64_t seed, double eps, int64_t *rowptr_out, int32_t *col_out);
+
+/*
  * Callers in front of the hot path (host side, one-off integer graph work; SURVEY.md §8f-2).
  * bigclam_conductance_seeds = conductanceLocalMin() (bigclam4-7.scala:58-73): ego-net conductance of every
  * node, candidates = the min-id neighbour of each node (tuple .min at :70), ranked by conductance ascending

@@ -16,7 +16,8 @@
 //   MBSGD()       bigclamv3-7.scala:206-222, Bigclamv2.scala:203-219   MBSGD(version)
 //   K sweep                                           :244-266   sweep_K()
 //   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta)
-//   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m)
+//   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m),
+//                                                                sample_graph(seed, eps)
 //
 // Errors: the reference throws JVM exceptions; here every negative return code of the C ABI becomes a bigclam::Error
 // (std::runtime_error carrying the code and bigclam_last_error()).  There is no CPU path: without a CUDA device
@@ -239,6 +240,21 @@ public:
         check(multi_ ? bigclam_multi_recommend(multi_, q, cnt, m, v.data(), x.data(), nullptr)
                      : bigclam_recommend(ctx_, q, cnt, m, v.data(), x.data(), nullptr),
               "recommend");
+    }
+    // A graph sampled from the model (bigclam_sample_graph): pairs that share a component are edges with probability
+    // p_uv (edge_probability's p), the others with probability eps; a symmetric CSR, rows ascending, the shape set_graph
+    // takes.  The same (F, seed, eps) gives the same graph.  Works for multi-GPU handles too.
+    void sample_graph(uint64_t seed, double eps, std::vector<int64_t> &rowptr, std::vector<int32_t> &col) {
+        need();
+        int64_t nnz = 0;
+        check(multi_ ? bigclam_multi_sample_graph_nnz(multi_, seed, eps, &nnz) : bigclam_sample_graph_nnz(ctx_, seed, eps, &nnz),
+              "sample_graph");
+        rowptr.assign((size_t)n_ + 1, 0);
+        col.assign((size_t)std::max<int64_t>(nnz, 1), 0);
+        check(multi_ ? bigclam_multi_sample_graph(multi_, seed, eps, rowptr.data(), col.data())
+                     : bigclam_sample_graph(ctx_, seed, eps, rowptr.data(), col.data()),
+              "sample_graph");
+        col.resize((size_t)nnz);
     }
 
     std::vector<int> Kset() const { return bigclam::Kset(minCom, maxCom, divCom); }
