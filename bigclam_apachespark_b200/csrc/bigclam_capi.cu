@@ -542,7 +542,7 @@ extern "C" int bigclam_create(bigclam_ctx **out, int64_t n, const int64_t *rowpt
         ctx->wide = sp_wide(ld);
         int sbps = 0, sb2 = 0;               // the grid must be resident for every variant (hub items wait for each other)
         if (ctx->wide) {
-            ctx->sp_wpb = kTlWarps;
+            ctx->sp_wpb = kTlWideWarps;
             ctx->sp_smem = sp_wide_block_smem_bytes(ld, ctx->sp_wpb);
             CUC(cudaFuncSetAttribute(tile_step_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));
             CUC(cudaFuncSetAttribute(tile_step_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->sp_smem));

@@ -59,11 +59,13 @@ constexpr int kTlMaxEdges = 32;
 #endif
 #define BIGCLAM_PRAGMA(x) _Pragma(#x)
 #define BIGCLAM_UNROLL(n) BIGCLAM_PRAGMA(unroll n)
+// one block of 13 warps per SM: with lcnt / loff inside fg (17.5 KB per warp at K = 200) and the block's steps and
+// sumF held once per SM, a 13th tile is in flight at K <= 256 (two blocks of 6 warps: 12)
 #ifndef BIGCLAM_TL_WARPS
-#define BIGCLAM_TL_WARPS 6
+#define BIGCLAM_TL_WARPS 13
 #endif
 #ifndef BIGCLAM_TL_BLOCKS
-#define BIGCLAM_TL_BLOCKS 2
+#define BIGCLAM_TL_BLOCKS 1
 #endif
 constexpr int kTlStage16 = BIGCLAM_TL_STAGE16;
 constexpr int kTlOwn16 = BIGCLAM_TL_OWN16;
@@ -74,25 +76,28 @@ constexpr int kTlErow = BIGCLAM_TL_EROW;
 constexpr int kTlWarps = BIGCLAM_TL_WARPS;
 constexpr int kTlBlocksPerSM = BIGCLAM_TL_BLOCKS;
 constexpr int kTlThreads = kTlWarps * 32;
+constexpr int kTlMbars = (kTlWarps + 1) & ~1;       // mbarrier slots: an even count keeps the warp regions 16-byte aligned
+constexpr int kTlWideWarps = 6;                      // warps per block of the wide variant (wide_step)
 static_assert(kTlStage16 >= 264, "the neighbour staging buffer doubles as xs[32 edges + 1 scratch row][16 trials]");
 static_assert(2 * kTlSlots >= 3 * kTlAct, "fg must hold (f, g) and sumF - f of the active components after compaction");
 static_assert(kTlEnt >= 128 && kTlEnt <= 256, "entry lists: the pair list (512 uint16) overlays ent_val; edge ids are bytes");
 static_assert(kTlAct <= 255, "active-component ids of the entry lists are bytes");
 static_assert(16 * kTlSlots >= 24 * kTlAct + 2 * 16 * kTlMaxEdges, "fg also holds sumF - f of the active components and the pair list of a line-search round");
+// behind the pair list, fg also holds the entry-list counters and offsets of phase I (lcnt, loff)
+constexpr int kTlLcntOff = 24 * kTlAct + 2 * 16 * kTlMaxEdges;
+static_assert(16 * kTlSlots >= kTlLcntOff + 4 * kTlAct + 2 * (kTlAct + 2), "fg also holds lcnt and loff behind the pair list");
 
 // per-warp shared memory of the tile path (W = ldp / 32 mask words per node)
 __host__ __device__ inline size_t tl_warp_bytes(int ld) {
     const size_t W = (size_t)sp_ldp(ld) / 32;
     size_t b = 16 * (size_t)kTlStage16;                 // stageN (later xs)
     b += 16 * (size_t)kTlOwn16;                         // stageO
-    b += 16 * (size_t)kTlSlots;                         // fg (later fa | asfm)
+    b += 16 * (size_t)kTlSlots;                         // fg (later fa | asfm | plist | lcnt | loff)
     b += 8 * (size_t)kTlEnt;                            // ent_val
     b += 8 * 32 + 8 * 8 + 8 * 8;                        // we, n_llh, n_G2
-    b += 4 * 2 * kTlMaxNodes * W + 4 * kTlMaxNodes;     // tmask, fmask, n_u
-    b += 4 * (size_t)kTlAct;                            // lcnt
+    b += 4 * kTlMaxNodes * W + 4 * kTlMaxNodes;         // tmask, n_u
     b += 2 * 2 * (size_t)kTlSlots;                      // slot_c (later ac), amap
-    b += 2 * ((size_t)kTlAct + 2);                      // loff
-    b += 2 * 2 * kTlMaxNodes * W;                       // pref_t, pref_f
+    b += 2 * kTlMaxNodes * W;                           // pref_t
     b += 2 * (40 + 40 + 12 + 12 + 12 + 8 + 8);          // e_soff, e_cnt, n_es, n_sb, n_ab, n_m, n_tot
     b += 2 * 32;                                        // e_io2
     b += 2 * (size_t)kTlEnt + 8 + 8;                    // ent_e, ent_a, n_js, n_want
@@ -104,9 +109,9 @@ __host__ __device__ inline size_t tl_region_bytes(int ld) {
     const size_t t = tl_warp_bytes(ld), g = (sp_gen_warp_bytes(ld) + 15) & ~(size_t)15;
     return t > g ? t : g;
 }
-// block: steps[kMaxSteps] | sumF[ldp] | mbar[kTlWarps] | wpb x warp region
+// block: steps[kMaxSteps] | sumF[ldp] | mbar[kTlMbars] | lns[16 floats] | wpb x warp region
 __host__ __device__ inline size_t tl_block_smem_bytes(int ld, int wpb) {
-    return sizeof(double) * (kMaxSteps + (size_t)sp_ldp(ld) + kTlWarps + 8) + (size_t)wpb * tl_region_bytes(ld);
+    return sizeof(double) * (kMaxSteps + (size_t)sp_ldp(ld) + kTlMbars + 8) + (size_t)wpb * tl_region_bytes(ld);
 }
 // warps per block: as many resident warps per SM as the shared memory (227 KB, 1 KB reserved per block) allows, in
 // at most kTlMaxBlocks blocks (wide rows run more blocks of fewer warps)
@@ -178,9 +183,9 @@ struct TlWarp {
     unsigned char *n_sl;
     int last_ns, last_nw;            // nodes of the last tile that were line-searched / that wanted a line search
     unsigned long long *mbar;
-    unsigned int *tmask, *fmask, *lcnt;
+    unsigned int *tmask, *lcnt;
     int *n_u;
-    unsigned short *slot_c, *amap, *loff, *plist, *pref_t, *pref_f, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_tot;
+    unsigned short *slot_c, *amap, *loff, *plist, *pref_t, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_tot;
     unsigned char *ent_e, *ent_a, *erow, *e_ni, *n_want;
     unsigned short *epos;
     signed char *n_js;
@@ -197,20 +202,18 @@ struct TlWarp {
         stageO = p;                                       p += 16 * (size_t)kTlOwn16;
         fg = reinterpret_cast<double2 *>(p);
         plist = reinterpret_cast<unsigned short *>(p + 24 * (size_t)kTlAct);   // (behind fa | asfm, after the compaction of the active components)
+        lcnt = reinterpret_cast<unsigned int *>(p + kTlLcntOff);                // (phase I, behind the pair list)
+        loff = reinterpret_cast<unsigned short *>(p + kTlLcntOff + 4 * (size_t)kTlAct);
         p += 16 * (size_t)kTlSlots;
         ent_val = reinterpret_cast<double *>(p);          p += 8 * (size_t)kTlEnt;
         we = reinterpret_cast<double *>(p);               p += 8 * 32;
         n_llh = reinterpret_cast<double *>(p);            p += 8 * 8;
         n_G2 = reinterpret_cast<double *>(p);             p += 8 * 8;
         tmask = reinterpret_cast<unsigned int *>(p);      p += 4 * (size_t)kTlMaxNodes * W;
-        fmask = reinterpret_cast<unsigned int *>(p);      p += 4 * (size_t)kTlMaxNodes * W;
         n_u = reinterpret_cast<int *>(p);                 p += 4 * kTlMaxNodes;
-        lcnt = reinterpret_cast<unsigned int *>(p);       p += 4 * (size_t)kTlAct;
         slot_c = reinterpret_cast<unsigned short *>(p);   p += 2 * (size_t)kTlSlots;
         amap = reinterpret_cast<unsigned short *>(p);     p += 2 * (size_t)kTlSlots;
-        loff = reinterpret_cast<unsigned short *>(p);     p += 2 * ((size_t)kTlAct + 2);
         pref_t = reinterpret_cast<unsigned short *>(p);   p += 2 * (size_t)kTlMaxNodes * W;
-        pref_f = reinterpret_cast<unsigned short *>(p);   p += 2 * (size_t)kTlMaxNodes * W;
         e_soff = reinterpret_cast<unsigned short *>(p);   p += 2 * 40;
         e_cnt = reinterpret_cast<unsigned short *>(p);    p += 2 * 40;
         e_io2 = reinterpret_cast<unsigned short *>(p);    p += 2 * 32;     // flat entry t of row e: its index is stageN (as uint16) [(e_io2[e] + t) mod 2^16]
@@ -311,7 +314,7 @@ struct TlWarp {
             n_want[lane] = (unsigned char)(do_ls && in_uset && nm.deg > 0);
         }
 #pragma unroll 1
-        for (int i = lane; i < nn * W; i += 32) { tmask[i] = 0u; fmask[i] = 0u; }
+        for (int i = lane; i < nn * W; i += 32) tmask[i] = 0u;
 #if BIGCLAM_TL_BULK
         if (total_e + total_u > 0) {
             fence_proxy_async();                         // this warp's earlier accesses to the buffers come first
@@ -354,16 +357,12 @@ struct TlWarp {
         for (int i = sub; i < cu_g; i += gs) {
             const int c = oi[i];
             const double val = ov[i];
-            atomicOr(fmask + gW + (c >> 5), 1u << (c & 31));
+            atomicOr(tmask + gW + (c >> 5), 1u << (c & 31));
             fusf = fma(val, s_sumF[c], fusf);
             fufu = fma(val, val, fufu);
         }
         fusf = group_sum(fusf, gs);
         fufu = group_sum(fufu, gs);
-        __syncwarp();
-#pragma unroll 1
-        for (int i = lane; i < nn * W; i += 32) tmask[i] = fmask[i];
-        __syncwarp();
         // ---------------- C1. components the neighbours' rows touch ----------------
         double *rv = reinterpret_cast<double *>(stageN + 16 * (size_t)soff_e);
         unsigned short *ri = sp_idx(rv, (uint32_t)ce);
@@ -1097,8 +1096,8 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     double *s_steps = reinterpret_cast<double *>(smem_raw);
     double *s_sumF = s_steps + kMaxSteps;
     unsigned long long *s_mbar = reinterpret_cast<unsigned long long *>(s_sumF + ldp);
-    float *s_lns = reinterpret_cast<float *>(s_mbar + kTlWarps);          // 16 floats
-    unsigned char *wbase = reinterpret_cast<unsigned char *>(s_mbar + kTlWarps + 8) + (size_t)wib * tl_region_bytes(ld);
+    float *s_lns = reinterpret_cast<float *>(s_mbar + kTlMbars);          // 16 floats
+    unsigned char *wbase = reinterpret_cast<unsigned char *>(s_mbar + kTlMbars + 8) + (size_t)wib * tl_region_bytes(ld);
 
 #pragma unroll 1
     for (int i = threadIdx.x; i < ldp; i += nthreads) s_sumF[i] = (i < ld) ? a.sumF[i] : 0.0;
