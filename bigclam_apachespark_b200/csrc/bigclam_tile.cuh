@@ -39,7 +39,7 @@ constexpr int kTlMaxEdges = 32;
 #ifndef BIGCLAM_TL_ACT              // active components of all nodes of a tile
 #define BIGCLAM_TL_ACT 160
 #endif
-#ifndef BIGCLAM_TL_ENT              // neighbour entries on active components (>= 128: the pair list lives there later)
+#ifndef BIGCLAM_TL_ENT              // neighbour entries on active components (<= BIGCLAM_TL_SLOTS - BIGCLAM_TL_ACT)
 #define BIGCLAM_TL_ENT 224
 #endif
 #ifndef BIGCLAM_TL_EROW             // neighbour entries of a tile (flat entry -> row map)
@@ -59,10 +59,10 @@ constexpr int kTlMaxEdges = 32;
 #endif
 #define BIGCLAM_PRAGMA(x) _Pragma(#x)
 #define BIGCLAM_UNROLL(n) BIGCLAM_PRAGMA(unroll n)
-// one block of 13 warps per SM: with lcnt / loff inside fg (17.5 KB per warp at K = 200) and the block's steps and
-// sumF held once per SM, a 13th tile is in flight at K <= 256 (two blocks of 6 warps: 12)
+// one block of 15 warps per SM at K <= 256: the line-search entry lists overlay buffers that are dead by then (15.2 KB
+// per warp at K = 200, see tl_lsov_bytes), and the block's steps and sumF are held once per SM
 #ifndef BIGCLAM_TL_WARPS
-#define BIGCLAM_TL_WARPS 13
+#define BIGCLAM_TL_WARPS 15
 #endif
 #ifndef BIGCLAM_TL_BLOCKS
 #define BIGCLAM_TL_BLOCKS 1
@@ -80,27 +80,36 @@ constexpr int kTlMbars = (kTlWarps + 1) & ~1;       // mbarrier slots: an even c
 constexpr int kTlWideWarps = 6;                      // warps per block of the wide variant (wide_step)
 static_assert(kTlStage16 >= 264, "the neighbour staging buffer doubles as xs[32 edges + 1 scratch row][16 trials]");
 static_assert(2 * kTlSlots >= 3 * kTlAct, "fg must hold (f, g) and sumF - f of the active components after compaction");
-static_assert(kTlEnt >= 128 && kTlEnt <= 256, "entry lists: the pair list (512 uint16) overlays ent_val; edge ids are bytes");
+static_assert(kTlEnt <= 256, "entry lists: edge ids are bytes");
 static_assert(kTlAct <= 255, "active-component ids of the entry lists are bytes");
 static_assert(16 * kTlSlots >= 24 * kTlAct + 2 * 16 * kTlMaxEdges, "fg also holds sumF - f of the active components and the pair list of a line-search round");
 // behind the pair list, fg also holds the entry-list counters and offsets of phase I (lcnt, loff)
 constexpr int kTlLcntOff = 24 * kTlAct + 2 * 16 * kTlMaxEdges;
 static_assert(16 * kTlSlots >= kTlLcntOff + 4 * kTlAct + 2 * (kTlAct + 2), "fg also holds lcnt and loff behind the pair list");
 
+// The entry lists of phases I-K overlay buffers that are dead by then:
+//   ent_val on stageO | we | tmask | pref_t  (stageO and tmask are last read in C2, pref_t in C2, we (as we2) in H2;
+//     at small K that span is shorter than ent_val, and the overlay takes the larger of the two);
+//   ent_e, ent_a on slot_c[kTlAct..kTlSlots)  (after the compaction in H, slot_c is read below A <= kTlAct - 1 only).
+static_assert(kTlSlots - kTlAct >= kTlEnt, "ent_e and ent_a (one byte per entry each) fit in slot_c behind the active components");
+__host__ __device__ inline size_t tl_lsov_bytes(int ld) {           // stageO | we | tmask | pref_t, overlaid by ent_val
+    const size_t W = (size_t)sp_ldp(ld) / 32;
+    const size_t span = 16 * (size_t)kTlOwn16 + 8 * 32 + 4 * kTlMaxNodes * W + 2 * kTlMaxNodes * W;
+    const size_t ev = 8 * (size_t)kTlEnt;
+    return ((span > ev ? span : ev) + 15) & ~(size_t)15;
+}
+
 // per-warp shared memory of the tile path (W = ldp / 32 mask words per node)
 __host__ __device__ inline size_t tl_warp_bytes(int ld) {
-    const size_t W = (size_t)sp_ldp(ld) / 32;
     size_t b = 16 * (size_t)kTlStage16;                 // stageN (later xs)
-    b += 16 * (size_t)kTlOwn16;                         // stageO
     b += 16 * (size_t)kTlSlots;                         // fg (later fa | asfm | plist | lcnt | loff)
-    b += 8 * (size_t)kTlEnt;                            // ent_val
-    b += 8 * 32 + 8 * 8 + 8 * 8;                        // we, n_llh, n_G2
-    b += 4 * kTlMaxNodes * W + 4 * kTlMaxNodes;         // tmask, n_u
-    b += 2 * 2 * (size_t)kTlSlots;                      // slot_c (later ac), amap
-    b += 2 * kTlMaxNodes * W;                           // pref_t
+    b += tl_lsov_bytes(ld);                             // stageO | we | tmask | pref_t (later ent_val)
+    b += 8 * 8 + 8 * 8;                                 // n_llh, n_G2
+    b += 4 * kTlMaxNodes;                               // n_u
+    b += 2 * 2 * (size_t)kTlSlots;                      // slot_c (later ac | ent_e | ent_a), amap
     b += 2 * (40 + 40 + 12 + 12 + 12 + 8 + 8);          // e_soff, e_cnt, n_es, n_sb, n_ab, n_m, n_tot
     b += 2 * 32;                                        // e_io2
-    b += 2 * (size_t)kTlEnt + 8 + 8;                    // ent_e, ent_a, n_js, n_want
+    b += 8 + 8;                                         // n_js, n_want
     b += (size_t)kTlErow + 2 * 34 + 32;                 // erow, epos, e_ni
     b += 2 * 8 + 8;                                     // n_sv, n_sl (line search by bounds)
     return (b + 15) & ~(size_t)15;
@@ -199,21 +208,27 @@ struct TlWarp {
         parity = 0;
         stageN = p;                                       p += 16 * (size_t)kTlStage16;
         xs = reinterpret_cast<double *>(stageN);          // (after the rows have been turned into per-component lists)
-        stageO = p;                                       p += 16 * (size_t)kTlOwn16;
         fg = reinterpret_cast<double2 *>(p);
         plist = reinterpret_cast<unsigned short *>(p + 24 * (size_t)kTlAct);   // (behind fa | asfm, after the compaction of the active components)
         lcnt = reinterpret_cast<unsigned int *>(p + kTlLcntOff);                // (phase I, behind the pair list)
         loff = reinterpret_cast<unsigned short *>(p + kTlLcntOff + 4 * (size_t)kTlAct);
         p += 16 * (size_t)kTlSlots;
-        ent_val = reinterpret_cast<double *>(p);          p += 8 * (size_t)kTlEnt;
-        we = reinterpret_cast<double *>(p);               p += 8 * 32;
+        {
+            unsigned char *q = p;                         // phases A-H2 ...
+            stageO = q;                                   q += 16 * (size_t)kTlOwn16;
+            we = reinterpret_cast<double *>(q);           q += 8 * 32;
+            tmask = reinterpret_cast<unsigned int *>(q);  q += 4 * (size_t)kTlMaxNodes * W;
+            pref_t = reinterpret_cast<unsigned short *>(q);
+            ent_val = reinterpret_cast<double *>(p);      // ... and phases I-K
+            p += tl_lsov_bytes(ld_);
+        }
         n_llh = reinterpret_cast<double *>(p);            p += 8 * 8;
         n_G2 = reinterpret_cast<double *>(p);             p += 8 * 8;
-        tmask = reinterpret_cast<unsigned int *>(p);      p += 4 * (size_t)kTlMaxNodes * W;
         n_u = reinterpret_cast<int *>(p);                 p += 4 * kTlMaxNodes;
         slot_c = reinterpret_cast<unsigned short *>(p);   p += 2 * (size_t)kTlSlots;
+        ent_e = reinterpret_cast<unsigned char *>(slot_c + kTlAct);       // (phases I-K: slot_c is read below A only by then)
+        ent_a = ent_e + kTlEnt;
         amap = reinterpret_cast<unsigned short *>(p);     p += 2 * (size_t)kTlSlots;
-        pref_t = reinterpret_cast<unsigned short *>(p);   p += 2 * (size_t)kTlMaxNodes * W;
         e_soff = reinterpret_cast<unsigned short *>(p);   p += 2 * 40;
         e_cnt = reinterpret_cast<unsigned short *>(p);    p += 2 * 40;
         e_io2 = reinterpret_cast<unsigned short *>(p);    p += 2 * 32;     // flat entry t of row e: its index is stageN (as uint16) [(e_io2[e] + t) mod 2^16]
@@ -223,8 +238,6 @@ struct TlWarp {
         n_m = reinterpret_cast<unsigned short *>(p);      p += 2 * 8;
         n_tot = reinterpret_cast<unsigned short *>(p);    p += 2 * 8;
         epos = reinterpret_cast<unsigned short *>(p);     p += 2 * 34;
-        ent_e = p;                                        p += (size_t)kTlEnt;
-        ent_a = p;                                        p += (size_t)kTlEnt;
         erow = p;                                         p += (size_t)kTlErow;
         e_ni = p;                                         p += 32;
         n_js = reinterpret_cast<signed char *>(p);        p += 8;
@@ -997,14 +1010,15 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                 pd += __popc(bd);
             }
         }
+        const uint64_t hu_g = __shfl_sync(0xffffffffu, hu, g);
         if (gv && js < 0) {
-            // row kept: block copy of the staged own row
-            const uint4 *src = reinterpret_cast<const uint4 *>(ov);
+            // row kept: block copy of the node's input row (the block phase A staged; stageO is overlaid by now)
+            const uint4 *src = reinterpret_cast<const uint4 *>(pool_in + sp_off8(hu_g));
             uint4 *dst = reinterpret_cast<uint4 *>(outv);
             const int q16 = wrow >> 1;
 #pragma unroll 1
             for (int q = sub; q < q16; q += gs) {
-                const uint4 blk = src[q];
+                const uint4 blk = __ldg(src + q);
                 dst[q] = blk;
                 if (kPush)
                     for (int pr = 0; pr < sp->n_peers; ++pr) reinterpret_cast<uint4 *>(sp->peer_pool[pr] + off)[q] = blk;
