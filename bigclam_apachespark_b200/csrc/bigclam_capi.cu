@@ -1983,6 +1983,199 @@ extern "C" int bigclam_sample_graph(bigclam_ctx *ctx, uint64_t seed, double eps,
 }
 
 // ------------------------------------------------------------------------------------------------
+// Fold-in (bigclam_sparse.cuh, fold_in_kernel): rows for new nodes with the fitted F and sumF held fixed.  Reads F only,
+// on the context's stream, like the calls above.
+static int fold_args_check(bigclam_ctx *ctx, const char *what, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter,
+                           double rel_tol, const void *out1, const void *out2, const void *out3) {
+    if (q < 0) return fail(ctx, BIGCLAM_EINVAL, "%s: q < 0", what);
+    if (max_iter < 1) return fail(ctx, BIGCLAM_EINVAL, "%s: max_iter = %d, must be >= 1", what, max_iter);
+    if (!(rel_tol >= 0.0)) return fail(ctx, BIGCLAM_EINVAL, "%s: rel_tol = %g, must be >= 0", what, rel_tol);
+    if (q == 0) return BIGCLAM_OK;
+    if (rowptr == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: rowptr is NULL", what);
+    if (rowptr[0] != 0) return fail(ctx, BIGCLAM_EINVAL, "%s: rowptr[0] = %lld, must be 0", what, (long long)rowptr[0]);
+    for (int64_t i = 0; i < q; ++i)
+        if (rowptr[i + 1] < rowptr[i]) return fail(ctx, BIGCLAM_EINVAL, "%s: rowptr decreases at %lld", what, (long long)i);
+    if (rowptr[q] > 0 && col == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: col is NULL", what);
+    if (int rc = check_ids(ctx, what, "col", col, rowptr[q])) return rc;
+    if (out1 == nullptr || out2 == nullptr || out3 == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: NULL output", what);
+    if (ctx->p.min_f != 0.0) return fail(ctx, BIGCLAM_EUNSUPPORTED, "%s: needs min_f == 0 (min_f = %g)", what, ctx->p.min_f);
+    return BIGCLAM_OK;
+}
+
+// Both calls.  Nodes with an empty list are answered here (zero row, l = 0, no steps).  The others go in chunks whose
+// lists fit the scratch bound (the smaller of 1 GiB and 10 % of the free memory; a longer list gets a chunk of its own),
+// and each chunk in batches whose rows fit it (a row is at most min(k, its neighbours' non-zeros) long).  fill == false:
+// only the row lengths, added up into *nnz_out.
+static int fold_in(bigclam_ctx *ctx, const char *what, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                   bool fill, int64_t *nnz_out, int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out) {
+    CU(cudaSetDevice(ctx->device));
+    const bigclam_params &p = ctx->p;
+    FoldArgs fa{};
+    fa.s = row_src(ctx);
+    fa.sumF = ctx->d_sumF[ctx->cur];
+    fa.ec = EdgeConst{-std::log(p.max_p) * (1.0 - 1e-12), -std::log(p.min_p) * (1.0 + 1e-12), std::log(1.0 - p.max_p),
+                      std::log(1.0 - p.min_p), 1.0 / (1.0 - p.max_p), 1.0 / (1.0 - p.min_p)};      // (fill_args)
+    for (int i = 0; i < kMaxSteps; ++i) fa.steps[i] = i < ctx->nsteps ? ctx->steps[i] : 0.0;
+    fa.nsteps = ctx->nsteps;
+    fa.alpha = p.alpha;
+    fa.max_f = p.max_f;
+    fa.max_iter = max_iter;
+    fa.rel_tol = rel_tol;
+    SparseArgs sp{};
+    sp.hdr_in = fa.s.hdr;
+    sp.pool_in = fa.s.pool;
+    const bool wide = sp_wide(fa.s.ld);
+    const size_t wb = fold_warp_bytes(fa.s.ld);
+    {
+        std::vector<double> sf((size_t)p.k);
+        CU(cudaMemcpyAsync(sf.data(), fa.sumF, sizeof(double) * (size_t)p.k, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        double s2 = 0.0;
+        for (double v : sf) s2 += v * v;
+        fa.S2_all = s2;
+    }
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    int64_t budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    if (const char *e = std::getenv("BIGCLAM_FOLD_IN_BUDGET")) budget = std::max<int64_t>(1, std::atoll(e));   // (tests: many batches)
+    // wide rows: the per-warp vectors of the whole grid, zeroed once (the kernel leaves them at zero)
+    int64_t grid_blocks = (int64_t)ctx->num_sms * 2;
+    DevBuf<unsigned char> scratch;
+    if (wide) {
+        grid_blocks = std::max<int64_t>(1, std::min<int64_t>(grid_blocks, budget / 2 / (kFoldWarps * (int64_t)wb)));
+        const size_t sbytes = (size_t)grid_blocks * kFoldWarps * wb;
+        if (scratch.reserve(sbytes) != cudaSuccess)
+            return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for the %lld-byte scratch of one block", what, (long long)(kFoldWarps * wb));
+        CU(cudaMemsetAsync(scratch.p, 0, sbytes, ctx->stream));
+        fa.scratch = scratch.p;
+    } else {
+        CU(cudaFuncSetAttribute(fold_in_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kFoldWarps * wb)));
+    }
+    int64_t nnz = 0;
+    if (fill) indptr_out[0] = 0;
+    DevBuf<int64_t> drp, dbound, dslot;
+    DevBuf<int32_t> dcol, dcnt, diters, didx;
+    DevBuf<double> dllh, dval;
+    std::vector<int64_t> hrp, hbound, hslot;
+    std::vector<int32_t> hcnt, hiters, hidx;
+    std::vector<double> hllh, hval;
+    for (int64_t c0 = 0; c0 < q;) {
+        // a chunk: consecutive nodes whose lists (4 bytes an entry) and per-node records (64 bytes) fit half the bound
+        int64_t c1 = c0 + 1;
+        while (c1 < q && c1 - c0 < ((int64_t)1 << 20) && 4 * (rowptr[c1 + 1] - rowptr[c0]) + 64 * (c1 + 1 - c0) <= budget / 2) ++c1;
+        const int64_t nc = c1 - c0, ec = rowptr[c1] - rowptr[c0];
+        if (dcol.reserve((size_t)ec) != cudaSuccess) {
+            if (nc == 1) return fail(ctx, BIGCLAM_ENOMEM, "%s: node %lld has %lld neighbours; no room for their list", what, (long long)c0, (long long)ec);
+            return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte chunk of lists", what, (long long)(4 * ec));
+        }
+        CU(drp.reserve((size_t)nc + 1));
+        CU(dbound.reserve((size_t)nc));
+        CU(dcnt.reserve((size_t)nc));
+        CU(dllh.reserve((size_t)nc));
+        CU(diters.reserve((size_t)nc));
+        CU(dslot.reserve((size_t)nc + 1));
+        hrp.resize((size_t)nc + 1);
+        for (int64_t i = 0; i <= nc; ++i) hrp[(size_t)i] = rowptr[c0 + i] - rowptr[c0];
+        CU(cudaMemcpyAsync(drp.p, hrp.data(), sizeof(int64_t) * ((size_t)nc + 1), cudaMemcpyHostToDevice, ctx->stream));
+        if (ec > 0) CU(cudaMemcpyAsync(dcol.p, col + rowptr[c0], sizeof(int32_t) * (size_t)ec, cudaMemcpyHostToDevice, ctx->stream));
+        hbound.resize((size_t)nc);
+        if (fill) {
+            fold_bound_kernel<<<(unsigned)((nc + 3) / 4), 128, 0, ctx->stream>>>(fa.s, drp.p, dcol.p, nc, dbound.p);
+            CU(cudaGetLastError());
+            CU(cudaMemcpyAsync(hbound.data(), dbound.p, sizeof(int64_t) * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaStreamSynchronize(ctx->stream));
+        }
+        hcnt.assign((size_t)nc, 0);
+        hllh.assign((size_t)nc, 0.0);
+        hiters.assign((size_t)nc, 0);
+        for (int64_t b0 = 0; b0 < nc;) {
+            // a batch: the chunk's nodes whose rows (12 bytes an entry) fit the other half of the bound
+            int64_t b1 = b0, total = 0;
+            hslot.resize((size_t)nc + 1);
+            hslot[0] = 0;
+            while (b1 < nc && (b1 == b0 || !fill || 12 * (total + hbound[(size_t)b1]) <= budget / 2)) {
+                total += fill ? hbound[(size_t)b1] : 0;
+                hslot[(size_t)(b1 - b0 + 1)] = total;
+                ++b1;
+            }
+            const int64_t nb = b1 - b0;
+            if (hrp[(size_t)b1] > hrp[(size_t)b0]) {        // (a batch of empty lists needs no device work)
+                fa.rowptr = drp.p + b0;
+                fa.col = dcol.p;
+                fa.nq = nb;
+                fa.cnt = dcnt.p + b0;
+                fa.llh = dllh.p + b0;
+                fa.iters = diters.p + b0;
+                fa.slot = nullptr;
+                if (fill) {
+                    if (didx.reserve((size_t)total) != cudaSuccess || dval.reserve((size_t)total) != cudaSuccess) {
+                        if (nb == 1) return fail(ctx, BIGCLAM_ENOMEM, "%s: node %lld: no room for its %lld-entry row", what, (long long)(c0 + b0), (long long)total);
+                        return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte batch of rows", what, (long long)(12 * total));
+                    }
+                    CU(cudaMemcpyAsync(dslot.p, hslot.data(), sizeof(int64_t) * ((size_t)nb + 1), cudaMemcpyHostToDevice, ctx->stream));
+                    fa.slot = dslot.p;
+                    fa.out_idx = didx.p;
+                    fa.out_val = dval.p;
+                }
+                if (wide) {
+                    const unsigned grid = (unsigned)std::min<int64_t>((nb + kFoldWarps - 1) / kFoldWarps, grid_blocks);
+                    fold_in_kernel<true><<<grid, kFoldWarps * 32, 0, ctx->stream>>>(fa, sp);
+                } else {
+                    fold_in_kernel<false><<<(unsigned)((nb + kFoldWarps - 1) / kFoldWarps), kFoldWarps * 32, kFoldWarps * wb, ctx->stream>>>(fa, sp);
+                }
+                CU(cudaGetLastError());
+                CU(cudaMemcpyAsync(hcnt.data() + b0, dcnt.p + b0, sizeof(int32_t) * (size_t)nb, cudaMemcpyDeviceToHost, ctx->stream));
+                CU(cudaMemcpyAsync(hllh.data() + b0, dllh.p + b0, sizeof(double) * (size_t)nb, cudaMemcpyDeviceToHost, ctx->stream));
+                CU(cudaMemcpyAsync(hiters.data() + b0, diters.p + b0, sizeof(int32_t) * (size_t)nb, cudaMemcpyDeviceToHost, ctx->stream));
+                if (fill && total > 0) {
+                    hidx.resize((size_t)total);
+                    hval.resize((size_t)total);
+                    CU(cudaMemcpyAsync(hidx.data(), didx.p, sizeof(int32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+                    CU(cudaMemcpyAsync(hval.data(), dval.p, sizeof(double) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+                }
+                CU(cudaStreamSynchronize(ctx->stream));
+            }
+            for (int64_t i = b0; i < b1; ++i) {
+                const int64_t u = c0 + i, cu = hcnt[(size_t)i];
+                if (fill) {
+                    const int64_t src = hslot[(size_t)(i - b0)];
+                    std::copy(hidx.begin() + src, hidx.begin() + src + cu, indices_out + nnz);
+                    std::copy(hval.begin() + src, hval.begin() + src + cu, values_out + nnz);
+                    indptr_out[u + 1] = nnz + cu;
+                    if (llh_out != nullptr) llh_out[u] = hllh[(size_t)i];
+                    if (iters_out != nullptr) iters_out[u] = hiters[(size_t)i];
+                }
+                nnz += cu;
+            }
+            b0 = b1;
+        }
+        c0 = c1;
+    }
+    if (nnz_out != nullptr) *nnz_out = nnz;
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_fold_in_nnz(bigclam_ctx *ctx, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                                   int64_t *nnz_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_fold_in_nnz";
+    if (int rc = fold_args_check(ctx, what, q, rowptr, col, max_iter, rel_tol, nnz_out, nnz_out, nnz_out)) return rc;
+    if (nnz_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: nnz_out is NULL", what);
+    *nnz_out = 0;
+    if (q == 0) return BIGCLAM_OK;
+    return fold_in(ctx, what, q, rowptr, col, max_iter, rel_tol, false, nnz_out, nullptr, nullptr, nullptr, nullptr, nullptr);
+}
+
+extern "C" int bigclam_fold_in(bigclam_ctx *ctx, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                               int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_fold_in";
+    if (int rc = fold_args_check(ctx, what, q, rowptr, col, max_iter, rel_tol, indptr_out, indices_out, values_out)) return rc;
+    if (q == 0) return BIGCLAM_OK;
+    return fold_in(ctx, what, q, rowptr, col, max_iter, rel_tol, true, nullptr, indptr_out, indices_out, values_out, llh_out, iters_out);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Fused collective of the node-partitioned path: exchange buffers (see bigclam_ctx::x_*).
 static int xchg_alloc(bigclam_ctx *ctx, int32_t world, int32_t rank) {
     if (world < 1 || world > 8 || rank < 0 || rank >= world) return fail(ctx, BIGCLAM_EINVAL, "exchange buffers: bad world/rank (at most 8 GPUs)");
@@ -2232,6 +2425,18 @@ extern "C" int bigclam_multi_sample_graph_nnz(bigclam_multi *m, uint64_t seed, d
 extern "C" int bigclam_multi_sample_graph(bigclam_multi *m, uint64_t seed, double eps, int64_t *rowptr_out, int32_t *col_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     MCALL(bigclam_sample_graph(m->r[0], seed, eps, rowptr_out, col_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_fold_in_nnz(bigclam_multi *m, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter,
+                                         double rel_tol, int64_t *nnz_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_fold_in_nnz(m->r[0], q, rowptr, col, max_iter, rel_tol, nnz_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_fold_in(bigclam_multi *m, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                                     int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_fold_in(m->r[0], q, rowptr, col, max_iter, rel_tol, indptr_out, indices_out, values_out, llh_out, iters_out), m->r[0]);
     return BIGCLAM_OK;
 }
 

@@ -414,6 +414,39 @@ class BigClam:
             check(lib.bigclam_sample_graph(self._ctx, seed, eps, rowptr.ctypes.data, col.ctypes.data), self._ctx)
         return rowptr, col[:nnz.value]
 
+    def fold_in(self, rowptr, col, max_iter: int = 100, rel_tol: float = 1e-4):
+        """Rows for NEW nodes with the fitted F and sumF held fixed (the `transform` of the fit), on the GPU.  Query node i
+        has the neighbour list col[rowptr[i]:rowptr[i + 1]] among the fitted nodes; from a zero row, up to max_iter of the
+        reference's line searches on its own objective, stopping when none passes or the LLH gains less than rel_tol
+        (relative).  Nodes never see each other.  Returns (indptr int64[q + 1], indices int32[nnz], values float64[nnz],
+        llh float64[q], iters int32[q]): rows ascending without zeros, the shape set_F_csr takes."""
+        lib = _lib.load()
+        rowptr = np.ascontiguousarray(rowptr, dtype=np.int64).ravel()
+        col = np.ascontiguousarray(col, dtype=np.int32).ravel()
+        if len(rowptr) < 1:
+            raise ValueError("rowptr needs q + 1 >= 1 entries")
+        q = len(rowptr) - 1
+        if rowptr[-1] > len(col):
+            raise ValueError("rowptr[-1] is beyond col")
+        max_iter, rel_tol = int(max_iter), float(rel_tol)
+        nnz = C.c_int64()
+        args = (q, rowptr.ctypes.data, col.ctypes.data, max_iter, rel_tol)
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_fold_in_nnz(self._multi, *args, C.byref(nnz)))
+        else:
+            check(lib.bigclam_fold_in_nnz(self._need(), *args, C.byref(nnz)), self._ctx)
+        indptr = np.zeros(q + 1, dtype=np.int64)
+        indices = np.empty(max(nnz.value, 1), dtype=np.int32)
+        values = np.empty(max(nnz.value, 1), dtype=np.float64)
+        llh = np.zeros(q, dtype=np.float64)
+        iters = np.zeros(q, dtype=np.int32)
+        outs = (indptr.ctypes.data, indices.ctypes.data, values.ctypes.data, llh.ctypes.data, iters.ctypes.data)
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_fold_in(self._multi, *args, *outs))
+        else:
+            check(lib.bigclam_fold_in(self._ctx, *args, *outs), self._ctx)
+        return indptr, indices[:nnz.value], values[:nnz.value], llh, iters
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

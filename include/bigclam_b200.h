@@ -336,6 +336,44 @@ int bigclam_multi_sample_graph_nnz(bigclam_multi *m, uint64_t seed, double eps, 
 int bigclam_multi_sample_graph(bigclam_multi *m, uint64_t seed, double eps, int64_t *rowptr_out, int32_t *col_out);
 
 /*
+ * Fold-in: the rows of q NEW nodes (arrived after the fit), with the context's F and sumF held fixed.  Query node u
+ * comes with its neighbour list among the n fitted nodes, as a CSR: rowptr (q + 1) and col (rowptr[q] ids in [0, n));
+ * repeats and any order are allowed, as in bigclam_create.  Its objective is the step's (bigclam4-7.scala:157-184) for u
+ * appended to the graph, with every other row fixed:
+ *   l_u(f) = sum_{v in N(u)} [log(1 - clamp(exp(-f.F_v), min_p, max_p)) + f.F_v] - f.sumF
+ * (sumF the fitted one; the candidates are scored with sumF - f_old + f_new as at :176-180).  For each query node on its
+ * own:
+ *   start from f_0 = 0, l_0 = l_u(0);  for t = 1 .. max_iter: the reference's line search from f_{t-1} over the step
+ *   sizes of bigclam_step_sizes(beta, max_inter), candidates clamp(f + s g, 0, max_f), keeping the largest s with
+ *   l_u(cand) >= l_{t-1} + alpha s |g|^2 (|g|^2 over all k components, :181).  No candidate passes: stop at f_{t-1}.
+ *   Otherwise f_t = the candidate; stop if |1 - l_t / l_{t-1}| < rel_tol (:237 for one node).
+ * iters = the number of accepted steps; the row returned is the last one accepted, llh = l_u of it.  A node with an
+ * empty list gets a zero row, llh = 0 and iters = 0.  Query nodes never see each other: a node's results are the same
+ * bits whatever the other nodes of the call, their order or the batches they are cut into.
+ *
+ * The rows come in bigclam_get_F_csr's form (indptr q + 1, ascending indices, no stored zeros), ready for
+ * bigclam_set_F_csr of a context over the extended graph.  bigclam_fold_in_nnz gives their total nnz; bigclam_fold_in
+ * fills indptr_out, indices_out and values_out (sized with that nnz; the rows are computed again, nothing is kept
+ * between the calls) and, optionally, llh_out (q) and iters_out (q).  Both read F only, like the calls above: no state
+ * changes (F, sumF, accepted indices, a speculative step), no dense n x k or q x k image, the context's stream,
+ * synchronous.  q < 0, max_iter < 1, rel_tol negative or NaN, a NULL required buffer, rowptr[0] != 0, a decreasing
+ * rowptr or an id outside [0, n) give BIGCLAM_EINVAL before any device work; a context with min_f != 0 gives
+ * BIGCLAM_EUNSUPPORTED.  q == 0 is a no-op (nnz 0).  The nodes go in batches whose scratch stays within the smaller of
+ * 1 GiB and 10 % of the free device memory (a node that needs more gets a batch of its own); BIGCLAM_ENOMEM, naming the
+ * node, when even that cannot be allocated.
+ */
+int bigclam_fold_in_nnz(bigclam_ctx *ctx, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                        int64_t *nnz_out);
+int bigclam_fold_in(bigclam_ctx *ctx, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                    int64_t *indptr_out /* q + 1 */, int32_t *indices_out, double *values_out,
+                    double *llh_out /* q, optional: l_u of the returned row */, int32_t *iters_out /* q, optional */);
+/* The same for a multi-GPU handle: rank 0's replica is read, errors go to bigclam_multi_last_error. */
+int bigclam_multi_fold_in_nnz(bigclam_multi *m, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter,
+                              double rel_tol, int64_t *nnz_out);
+int bigclam_multi_fold_in(bigclam_multi *m, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
+                          int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out);
+
+/*
  * Callers in front of the hot path (host side, one-off integer graph work; SURVEY.md §8f-2).
  * bigclam_conductance_seeds = conductanceLocalMin() (bigclam4-7.scala:58-73): ego-net conductance of every
  * node, candidates = the min-id neighbour of each node (tuple .min at :70), ranked by conductance ascending

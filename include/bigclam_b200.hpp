@@ -18,6 +18,7 @@
 //   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta)
 //   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m),
 //                                                                sample_graph(seed, eps)
+//   rows for new nodes, the fit held fixed (:157-184 per node)    fold_in(rowptr, col, max_iter, rel_tol, ...)
 //
 // Errors: the reference throws JVM exceptions; here every negative return code of the C ABI becomes a bigclam::Error
 // (std::runtime_error carrying the code and bigclam_last_error()).  There is no CPU path: without a CUDA device
@@ -255,6 +256,33 @@ public:
                      : bigclam_sample_graph(ctx_, seed, eps, rowptr.data(), col.data()),
               "sample_graph");
         col.resize((size_t)nnz);
+    }
+    // Rows for new nodes with the fitted F and sumF held fixed (bigclam_fold_in): query node i has the neighbour list
+    // col[rowptr[i] .. rowptr[i + 1]) among the fitted nodes.  The rows come as a CSR (indptr, indices, values: ascending,
+    // no zeros, the shape set_F_csr takes), with each row's LLH term and accepted steps.  Works for multi-GPU handles too.
+    void fold_in(const std::vector<int64_t> &rowptr, const std::vector<int32_t> &col, int32_t max_iter, double rel_tol,
+                 std::vector<int64_t> &indptr, std::vector<int32_t> &indices, std::vector<double> &values, std::vector<double> &llh,
+                 std::vector<int32_t> &iters) {
+        need();
+        if (rowptr.empty()) throw Error(BIGCLAM_EINVAL, "fold_in: rowptr needs q + 1 entries");
+        const int64_t q = (int64_t)rowptr.size() - 1;
+        if (rowptr.back() > (int64_t)col.size()) throw Error(BIGCLAM_EINVAL, "fold_in: rowptr goes beyond col");
+        int64_t nnz = 0;
+        check(multi_ ? bigclam_multi_fold_in_nnz(multi_, q, rowptr.data(), col.data(), max_iter, rel_tol, &nnz)
+                     : bigclam_fold_in_nnz(ctx_, q, rowptr.data(), col.data(), max_iter, rel_tol, &nnz),
+              "fold_in");
+        indptr.assign((size_t)q + 1, 0);
+        indices.assign((size_t)std::max<int64_t>(nnz, 1), 0);
+        values.assign((size_t)std::max<int64_t>(nnz, 1), 0.0);
+        llh.assign((size_t)q, 0.0);
+        iters.assign((size_t)q, 0);
+        check(multi_ ? bigclam_multi_fold_in(multi_, q, rowptr.data(), col.data(), max_iter, rel_tol, indptr.data(), indices.data(),
+                                             values.data(), llh.data(), iters.data())
+                     : bigclam_fold_in(ctx_, q, rowptr.data(), col.data(), max_iter, rel_tol, indptr.data(), indices.data(), values.data(),
+                                       llh.data(), iters.data()),
+              "fold_in");
+        indices.resize((size_t)nnz);
+        values.resize((size_t)nnz);
     }
 
     std::vector<int> Kset() const { return bigclam::Kset(minCom, maxCom, divCom); }
