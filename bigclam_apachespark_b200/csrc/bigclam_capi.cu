@@ -1006,6 +1006,13 @@ extern "C" int bigclam_get_accepted(bigclam_ctx *ctx, int8_t *accepted_out) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// The thresholds and constants of the clamped edge term (edge_term, pair_p):
+// exp(-x) >= max_p  <=>  x <= -log(max_p);  exp(-x) <= min_p  <=>  x >= -log(min_p)
+static EdgeConst edge_const(const bigclam_params &p) {
+    return EdgeConst{-std::log(p.max_p) * (1.0 - 1e-12), -std::log(p.min_p) * (1.0 + 1e-12), std::log(1.0 - p.max_p),
+                     std::log(1.0 - p.min_p), 1.0 / (1.0 - p.max_p), 1.0 / (1.0 - p.min_p)};
+}
+
 static void fill_args(bigclam_ctx *ctx, StepArgs &a, bool linesearch, const uint8_t *d_mask, bool use_done) {
     const bigclam_params &p = ctx->p;
     a.n = ctx->n;
@@ -1020,13 +1027,8 @@ static void fill_args(bigclam_ctx *ctx, StepArgs &a, bool linesearch, const uint
     for (int i = 0; i < kMaxSteps; ++i) a.steps[i] = i < ctx->nsteps ? ctx->steps[i] : 0.0;
     a.alpha = p.alpha;
     a.min_p = p.min_p; a.max_p = p.max_p; a.min_f = p.min_f; a.max_f = p.max_f;
-    // exp(-x) >= max_p  <=>  x <= -log(max_p);  exp(-x) <= min_p  <=>  x >= -log(min_p)
-    a.x_lo = -std::log(p.max_p) * (1.0 - 1e-12);
-    a.x_hi = -std::log(p.min_p) * (1.0 + 1e-12);
-    a.t_lo = std::log(1.0 - p.max_p);
-    a.t_hi = std::log(1.0 - p.min_p);
-    a.w_lo = 1.0 / (1.0 - p.max_p);
-    a.w_hi = 1.0 / (1.0 - p.min_p);
+    const EdgeConst ec = edge_const(p);
+    a.x_lo = ec.x_lo; a.x_hi = ec.x_hi; a.t_lo = ec.t_lo; a.t_hi = ec.t_hi; a.w_lo = ec.w_lo; a.w_hi = ec.w_hi;
     a.meta = ctx->d_meta;
     a.work_counter = ctx->d_work;
     a.n_peers = linesearch ? ctx->n_peers : 0;
@@ -1758,7 +1760,17 @@ static RowSrc row_src(const bigclam_ctx *ctx) {
 }
 
 static PairConst pair_const(const bigclam_ctx *ctx) {
-    return PairConst{ctx->p.min_p, ctx->p.max_p, -std::log(ctx->p.max_p) * (1.0 - 1e-12), -std::log(ctx->p.min_p) * (1.0 + 1e-12)};
+    const EdgeConst ec = edge_const(ctx->p);
+    return PairConst{ctx->p.min_p, ctx->p.max_p, ec.x_lo, ec.x_hi};
+}
+
+// Scratch bound of the read-only queries (recommend, sample_graph, fold_in): the smaller of 1 GiB and 10 % of the free
+// memory.
+static cudaError_t query_budget(int64_t &budget) {
+    size_t free_b = 0, total_b = 0;
+    const cudaError_t e = cudaMemGetInfo(&free_b, &total_b);
+    budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    return e;
 }
 
 static int check_ids(bigclam_ctx *ctx, const char *what, const char *name, const int32_t *ids, int64_t count) {
@@ -1812,11 +1824,10 @@ extern "C" int bigclam_recommend(bigclam_ctx *ctx, const int32_t *nodes, int64_t
         if (int rc = check_ids(ctx, what, "nodes", nodes, count)) return rc;
     CU(cudaSetDevice(ctx->device));
     const RowSrc s = row_src(ctx);
-    // scratch bound: the smaller of 1 GiB and 10 % of the free memory, for the two-hop keys of a batch of nodes; a node
-    // whose list alone is longer gets a batch of its own with scratch sized for it
-    size_t free_b = 0, total_b = 0;
-    CU(cudaMemGetInfo(&free_b, &total_b));
-    const int64_t budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    // scratch bound (query_budget) for the two-hop keys of a batch of nodes; a node whose list alone is longer gets a
+    // batch of its own with scratch sized for it
+    int64_t budget;
+    CU(query_budget(budget));
     const int64_t budget_keys = std::max<int64_t>(1, budget / (int64_t)sizeof(uint32_t));
     const int64_t Q = std::max<int64_t>(1, std::min<int64_t>({count, (int64_t)1 << 16, budget / (12 * (int64_t)m + 64)}));   // nodes per chunk
     DevBuf<int32_t> dq, dv, dfound;
@@ -1952,11 +1963,10 @@ extern "C" int bigclam_sample_graph(bigclam_ctx *ctx, uint64_t seed, double eps,
     if (int rc = sample_count(ctx, seed, eps, pl, rowptr_out)) return rc;
     const int64_t n = ctx->n;
     if (rowptr_out[n] == 0) return BIGCLAM_OK;
-    // batches of consecutive rows whose output stays within the smaller of 1 GiB and 10 % of the free memory; a row
-    // longer than that alone gets a batch of its own
-    size_t free_b = 0, total_b = 0;
-    CU(cudaMemGetInfo(&free_b, &total_b));
-    const int64_t budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    // batches of consecutive rows whose output stays within the scratch bound (query_budget); a row longer than that
+    // alone gets a batch of its own
+    int64_t budget;
+    CU(query_budget(budget));
     const int64_t budget_entries = std::max<int64_t>(1, budget / (int64_t)sizeof(int32_t));
     DevBuf<int64_t> drowptr;
     DevBuf<int32_t> dout;
@@ -2003,22 +2013,16 @@ static int fold_args_check(bigclam_ctx *ctx, const char *what, int64_t q, const 
 }
 
 // Both calls.  Nodes with an empty list are answered here (zero row, l = 0, no steps).  The others go in chunks whose
-// lists fit the scratch bound (the smaller of 1 GiB and 10 % of the free memory; a longer list gets a chunk of its own),
-// and each chunk in batches whose rows fit it (a row is at most min(k, its neighbours' non-zeros) long).  fill == false:
-// only the row lengths, added up into *nnz_out.
+// lists fit the scratch bound (query_budget; a longer list gets a chunk of its own), and each chunk in batches whose
+// rows fit it (a row is at most min(k, its neighbours' non-zeros) long).  The kernel runs the step's own phases with
+// the context's step arguments (fill_args).  fill == false: only the row lengths, added up into *nnz_out.
 static int fold_in(bigclam_ctx *ctx, const char *what, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
                    bool fill, int64_t *nnz_out, int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out) {
     CU(cudaSetDevice(ctx->device));
-    const bigclam_params &p = ctx->p;
+    StepArgs a{};
+    fill_args(ctx, a, false, nullptr, false);
     FoldArgs fa{};
     fa.s = row_src(ctx);
-    fa.sumF = ctx->d_sumF[ctx->cur];
-    fa.ec = EdgeConst{-std::log(p.max_p) * (1.0 - 1e-12), -std::log(p.min_p) * (1.0 + 1e-12), std::log(1.0 - p.max_p),
-                      std::log(1.0 - p.min_p), 1.0 / (1.0 - p.max_p), 1.0 / (1.0 - p.min_p)};      // (fill_args)
-    for (int i = 0; i < kMaxSteps; ++i) fa.steps[i] = i < ctx->nsteps ? ctx->steps[i] : 0.0;
-    fa.nsteps = ctx->nsteps;
-    fa.alpha = p.alpha;
-    fa.max_f = p.max_f;
     fa.max_iter = max_iter;
     fa.rel_tol = rel_tol;
     SparseArgs sp{};
@@ -2027,16 +2031,15 @@ static int fold_in(bigclam_ctx *ctx, const char *what, int64_t q, const int64_t 
     const bool wide = sp_wide(fa.s.ld);
     const size_t wb = fold_warp_bytes(fa.s.ld);
     {
-        std::vector<double> sf((size_t)p.k);
-        CU(cudaMemcpyAsync(sf.data(), fa.sumF, sizeof(double) * (size_t)p.k, cudaMemcpyDeviceToHost, ctx->stream));
+        std::vector<double> sf((size_t)a.k);
+        CU(cudaMemcpyAsync(sf.data(), a.sumF, sizeof(double) * (size_t)a.k, cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
         double s2 = 0.0;
         for (double v : sf) s2 += v * v;
         fa.S2_all = s2;
     }
-    size_t free_b = 0, total_b = 0;
-    CU(cudaMemGetInfo(&free_b, &total_b));
-    int64_t budget = (int64_t)std::min<double>((double)((size_t)1 << 30), 0.1 * (double)free_b);
+    int64_t budget;
+    CU(query_budget(budget));
     if (const char *e = std::getenv("BIGCLAM_FOLD_IN_BUDGET")) budget = std::max<int64_t>(1, std::atoll(e));   // (tests: many batches)
     // wide rows: the per-warp vectors of the whole grid, zeroed once (the kernel leaves them at zero)
     int64_t grid_blocks = (int64_t)ctx->num_sms * 2;
@@ -2119,9 +2122,9 @@ static int fold_in(bigclam_ctx *ctx, const char *what, int64_t q, const int64_t 
                 }
                 if (wide) {
                     const unsigned grid = (unsigned)std::min<int64_t>((nb + kFoldWarps - 1) / kFoldWarps, grid_blocks);
-                    fold_in_kernel<true><<<grid, kFoldWarps * 32, 0, ctx->stream>>>(fa, sp);
+                    fold_in_kernel<true><<<grid, kFoldWarps * 32, 0, ctx->stream>>>(a, fa, sp);
                 } else {
-                    fold_in_kernel<false><<<(unsigned)((nb + kFoldWarps - 1) / kFoldWarps), kFoldWarps * 32, kFoldWarps * wb, ctx->stream>>>(fa, sp);
+                    fold_in_kernel<false><<<(unsigned)((nb + kFoldWarps - 1) / kFoldWarps), kFoldWarps * 32, kFoldWarps * wb, ctx->stream>>>(a, fa, sp);
                 }
                 CU(cudaGetLastError());
                 CU(cudaMemcpyAsync(hcnt.data() + b0, dcnt.p + b0, sizeof(int32_t) * (size_t)nb, cudaMemcpyDeviceToHost, ctx->stream));

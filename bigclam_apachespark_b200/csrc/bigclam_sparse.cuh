@@ -201,14 +201,23 @@ __device__ __forceinline__ void ls_code_near(double x, double x_lo, double En, f
     Lp = -1000.0f - vnear;
 }
 
+struct RowSrc {                    // the rows of the current F: sparse (hdr, pool) when hdr != nullptr, else dense (F, ld)
+    const uint64_t *hdr;
+    const double *pool;
+    const double *F;
+    int32_t k, ld;
+};
+
 // ---------------------------------------------------------------------------------------------------------------
 // The general path: everything one warp needs to process one node (or one hub item).  kWide: wide rows (see the
 // header comment): K-sized vectors in global scratch, sumF in global memory, touched-only per-node passes.
-template <bool kWide>
+// kFold: the phases as fold-in runs them (FoldGen): rows from `rs`, sparse or dense, and sumF' = sumF + f.
+template <bool kWide, bool kFold = false>
 struct SpGen {
     // launch-wide
     const StepArgs *a;
     const SparseArgs *sp;
+    const RowSrc *rs;                // fold-in: the fitted rows
     const double *s_steps;
     const double *s_sumF;            // (wide rows: the global sumF)
     const float *s_lns;              // upper bounds of ln(step size), 16 values (line search by bounds)
@@ -239,9 +248,7 @@ struct SpGen {
         poff = reinterpret_cast<unsigned short *>(cbal + sp_ldp(ecap) / 32);
         ccum = poff + 40;
     }
-    __device__ __forceinline__ void touch(int c) {
-        if constexpr (kWide) atomicOr(tmask + (c >> 5), 1u << (c & 31));
-    }
+    __device__ __forceinline__ void touch(int c) { atomicOr(tmask + (c >> 5), 1u << (c & 31)); }
 
     __device__ __forceinline__ void carve(unsigned char *wbase, int ld_, int lane_) {
         ld = ld_;
@@ -309,16 +316,53 @@ struct SpGen {
         __syncwarp();
         return ne;
     }
+    // Fold-in over dense rows: the same, each row compacted to its non-zeros by the whole warp, row after row, while
+    // the rows fit.
+    __device__ __forceinline__ int stage_dense(const int32_t *__restrict__ colp, int cnt32) {
+        int total = 0, ne = 0;
+        if (lane == 0) poff[0] = 0;
+#pragma unroll 1
+        for (; ne < cnt32; ++ne) {
+            const double *row = rs->F + (size_t)colp[ne] * rs->ld;
+            int cv = 0;
+#pragma unroll 1
+            for (int c0 = 0; c0 < rs->k; c0 += 32)
+                cv += __popc(__ballot_sync(0xffffffffu, c0 + lane < rs->k && __ldg(row + c0 + lane) != 0.0));
+            if (total + cv > ecap) break;                 // (never for the first row: k <= ecap)
+#pragma unroll 1
+            for (int c0 = 0; c0 < rs->k; c0 += 32) {
+                const int c = c0 + lane;
+                const double v = (c < rs->k) ? __ldg(row + c) : 0.0;
+                const unsigned bal = __ballot_sync(0xffffffffu, v != 0.0);
+                if (v != 0.0) {
+                    const int p = total + __popc(bal & lt_mask);
+                    ent_val[p] = v;
+                    ent_idx[p] = (unsigned short)c;
+                }
+                total += __popc(bal);
+            }
+            if (lane == 0) poff[ne + 1] = (unsigned short)total;
+        }
+        __syncwarp();
+        return ne;
+    }
+    __device__ __forceinline__ int stage(const int32_t *colp, int cnt32) {
+        if constexpr (kFold)
+            if (rs->hdr == nullptr) return stage_dense(colp, cnt32);
+        return stage_chunk(colp, cnt32);
+    }
 
     // PRE over the edges [eb, ee) of a node whose fu is in fu_d: returns this lane's share of S1 (lane e holds the
-    // terms of the chunks' e-th rows); with `axpy` the weighted neighbour rows are added into g_d.
-    __device__ __forceinline__ double pre_range(const int32_t *colbase, int eb, int ee, bool axpy, int &nchunks, int &ne_last) {
+    // terms of the chunks' e-th rows); with `axpy` the weighted neighbour rows are added into g_d, and with `mark`
+    // their components are set in tmask.
+    __device__ __forceinline__ double pre_range(const int32_t *colbase, int eb, int ee, bool axpy, int &nchunks, int &ne_last,
+                                                bool mark = kWide) {
         double S1 = 0.0;
         nchunks = 0;
         ne_last = 0;
 #pragma unroll 1
         for (int cb = eb; cb < ee;) {
-            const int ne = stage_chunk(colbase + cb, min(32, ee - cb));
+            const int ne = stage(colbase + cb, min(32, ee - cb));
             double x = 0.0;
             if (lane < ne) {
                 const int end = poff[lane + 1];
@@ -337,7 +381,7 @@ struct SpGen {
                     for (int i = pe + lane; i < pn; i += 32) {
                         const int c = ent_idx[i];
                         g_d[c] = fma(we, ent_val[i], g_d[c]);
-                        touch(c);
+                        if (mark) touch(c);
                     }
                     __syncwarp();
                 }
@@ -433,6 +477,67 @@ struct SpGen {
         __syncwarp();
         return (S2_all - SF2) + G2;
     }
+    // Fold-in: the components set in tmask, ascending, into `list` (once per node); returns their number.
+    __device__ __forceinline__ int list_touched(unsigned short *list) {
+        const int W = ldp >> 5;
+        int nt = 0;
+#pragma unroll 1
+        for (int w0 = 0; w0 < W; w0 += 32) {
+            const int w = w0 + lane;
+            unsigned bits = (w < W) ? tmask[w] : 0u;
+            const int pc = __popc(bits);
+            int incl = pc;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            int p = nt + incl - pc;
+            while (bits) {
+                list[p++] = (unsigned short)(32 * w + __ffs(bits) - 1);
+                bits &= bits - 1u;
+            }
+            nt += __shfl_sync(0xffffffffu, incl, 31);
+        }
+        __syncwarp();
+        return nt;
+    }
+    // Fold-in: scan_touched over the nt components of `list`, which is kept, with sumF' = sumF + f in the gradient.
+    // (The step keeps its own fused scan_touched: written as these two parts, its wide kernels compile to different
+    // instructions.)
+    __device__ __forceinline__ double scan_list(const unsigned short *list, int nt, int &m, bool &need_hi) {
+        double G2 = 0.0, SF2 = 0.0;
+        bool hi_lane = false;
+        m = 0;
+        const double max_f = a->max_f;
+#pragma unroll 1
+        for (int t0 = 0; t0 < nt; t0 += 32) {
+            const int t = t0 + lane;
+            const bool ok = t < nt;
+            const int c = ok ? (int)list[t] : 0;
+            double f = 0.0, g = 0.0;
+            if (ok) {
+                const double sf = __ldg(s_sumF + c);
+                f = fu_d[c];
+                g = (g_d[c] - (sf + f)) + f;
+                g_d[c] = g;
+                G2 = fma(g, g, G2);
+                SF2 = fma(sf, sf, SF2);
+            }
+            const bool act = ok && (f > 0.0 || g > 0.0);
+            const unsigned bal = __ballot_sync(0xffffffffu, act);
+            if (act) {
+                aidx[m + __popc(bal & lt_mask)] = (unsigned short)c;
+                hi_lane |= (f + g > max_f);
+            }
+            m += __popc(bal);
+        }
+        G2 = warp_sum(G2);
+        SF2 = warp_sum(SF2);
+        need_hi = __any_sync(0xffffffffu, hi_lane);
+        __syncwarp();
+        return (S2_all - SF2) + G2;
+    }
     // Wide rows: g_d of the touched components back to zero (when it was written) and the bitmask cleared.
     __device__ __forceinline__ void clear_touched(bool clear_g) {
         const int W = ldp >> 5;
@@ -490,7 +595,7 @@ struct SpGen {
         double sumterms = 0.0;
 #pragma unroll 1
         for (int cb = eb; cb < ee;) {
-            const int ne = (staged > 0) ? staged : stage_chunk(colbase + cb, min(32, ee - cb));
+            const int ne = (staged > 0) ? staged : stage(colbase + cb, min(32, ee - cb));
             compact_active(ne);
 #pragma unroll 1
             for (int e2 = 0; e2 < ne; e2 += 4) {
@@ -528,14 +633,14 @@ struct SpGen {
     __device__ __forceinline__ int decide(int tg, double s, bool jok, double sumterms, int m, bool need_hi, double llh_u, double G2, unsigned surv = 0xffffu) {
         const int h = lane >> 4;
         const double max_f = a->max_f;
-        // - newfu.sfT + newfu.newfu with sfT = (sumF - fu) + newfu   (:176,:180)
+        // - newfu.sfT + newfu.newfu with sfT = (sumF - fu) + newfu   (:176,:180; fold-in: sumF' = sumF + fu)
         double oa = 0.0, ob = 0.0;
 #pragma unroll 1
         for (int t = h; t < m; t += 2) {
             const int c = aidx[t];
             const double f = fu_d[c], g = g_d[c];
             const double nf = need_hi ? clamp_step0(f, s, g, max_f) : clamp_step0_lo(f, s, g);
-            const double sf = (s_sumF[c] - f) + nf;
+            const double sf = ((kFold ? __ldg(s_sumF + c) + f : s_sumF[c]) - f) + nf;
             oa = fma(nf, sf, oa);
             ob = fma(nf, nf, ob);
         }
@@ -646,7 +751,7 @@ struct SpGen {
             const double v = __ldg(uval + i);
             const int c = __ldg(uidx + i);
             fu_d[c] = v;
-            touch(c);
+            if constexpr (kWide) touch(c);
             fusf = fma(v, s_sumF[c], fusf);
             fufu = fma(v, v, fufu);
         }
@@ -1046,12 +1151,6 @@ __global__ void sparse_to_dense_kernel(const uint64_t *hdr, const double *pool, 
 // ascending c with every product and every sum rounded on its own: the same bits for sparse and dense rows, for (u, v)
 // and (v, u), and for a NumPy restatement.  p_uv = 1 - clamp(exp(-x), MIN_P_, MAX_P_), the clamp of
 // bigclam4-7.scala:166, so log(p_uv) + x_uv is the per-edge term of the LLH (:218).
-struct RowSrc {                    // the rows of the current F: sparse (hdr, pool) when hdr != nullptr, else dense (F, ld)
-    const uint64_t *hdr;
-    const double *pool;
-    const double *F;
-    int32_t k, ld;
-};
 struct PairConst {                 // the clamp of p, with the step kernel's exact shortcuts (fill_args)
     double min_p, max_p, x_lo, x_hi;
 };
@@ -1386,21 +1485,19 @@ __global__ void sample_rows_kernel(SampleArgs a, int64_t r0, int64_t r1, int64_t
 // most max_iter line searches over the 16 candidates, each taking the largest step that passes; it stops when none
 // passes or when |1 - l_t / l_{t-1}| < rel_tol (:237 for one node).
 //
-// One warp per query node, with the dense per-warp vectors fu_d / g_d of the general path, whose staging
-// (SpGen::stage_chunk) and active-entry compaction (SpGen::compact_active) it reuses; dense rows are staged by
-// stage() below.  Only the components the node TOUCHES (its neighbours' non-zeros; its own row stays inside them) are
-// visited: an untouched component has f = 0 and gradient -sumF_c <= 0, never moves, and enters |g|^2 through
-// S2_all - sum_touched sumF_c^2 (the identity of the tile and wide paths).  The touched list is built by the first PRE
-// and kept, ascending, for the node's whole run.  Every sum has a fixed order and there are no floating-point atomics:
-// a node's results are the same bits whatever the batch around it.
+// One warp per query node.  The phases are the general path's own, compiled for fold-in (SpGen<kWide, true>): PRE
+// (pre_range), the line search (ls_range) and the Armijo decision (decide), with the staging of sparse rows, a dense-row
+// stager and the active-entry compaction; the gradient scan over the touched components is SpGen::scan_list.  ptxas:
+// 80 registers (ld <= 1024) and 94 (wide rows), no spills.  Only the components the node TOUCHES
+// (its neighbours' non-zeros; its own row stays inside them) are visited: an untouched component has f = 0 and
+// gradient -sumF_c <= 0, never moves, and enters |g|^2 through S2_all - sum_touched sumF_c^2 (the identity of the tile
+// and wide paths).  The first PRE marks the touched components and they are listed once, ascending, in `tl` for the
+// node's whole run.  Every sum has a fixed order and there are no floating-point atomics: a node's results are the
+// same bits whatever the batch around it.  The step's constants (steps, alpha, max_f, the edge term's clamp) come
+// from the context's StepArgs; FoldArgs holds the batch.
 struct FoldArgs {
     RowSrc s;
-    const double *sumF;          // the fitted sumF (ld entries)
     double S2_all;               // sum_c sumF_c^2 over the k components, ascending c
-    EdgeConst ec;
-    double steps[kMaxSteps];
-    int32_t nsteps;
-    double alpha, max_f;
     const int64_t *rowptr;       // the batch's lists: node i has col[rowptr[i] .. rowptr[i + 1])
     const int32_t *col;
     int64_t nq;
@@ -1425,16 +1522,11 @@ __host__ __device__ inline size_t fold_warp_bytes(int ld) {
 
 template <bool kWide>
 struct FoldGen {
-    SpGen<kWide> g;              // staging of sparse rows and compaction of the staged entries (its other members unused)
+    SpGen<kWide, true> g;
     const FoldArgs *a;
-    unsigned int *tmask;         // touched components, one bit each
-    unsigned short *tl;          // ... and as an ascending list of nt
-    int nt;
+    unsigned short *tl;          // the touched components, ascending
 
-    __device__ __forceinline__ void carve(unsigned char *base, const SparseArgs *sp, const FoldArgs *fa, int lane) {
-        a = fa;
-        const int ld = fa->s.ld;
-        g.sp = sp;
+    __device__ __forceinline__ void carve(unsigned char *base, int ld, int lane) {
         g.ld = ld;
         g.ldp = sp_ldp(ld);
         g.ecap = sp_entries(ld);
@@ -1445,212 +1537,12 @@ struct FoldGen {
         g.g_d = g.fu_d + g.ldp;
         g.ent_val = g.g_d + g.ldp;
         g.cbal = reinterpret_cast<unsigned int *>(g.ent_val + g.ecap);
-        tmask = g.cbal + Ew;
-        g.tmask = tmask;
-        g.ent_idx = reinterpret_cast<unsigned short *>(tmask + g.ldp / 32);
+        g.tmask = g.cbal + Ew;
+        g.ent_idx = reinterpret_cast<unsigned short *>(g.tmask + g.ldp / 32);
         tl = g.ent_idx + g.ecap;
         g.aidx = tl + g.ldp;
         g.poff = g.aidx + g.ldp;
         g.ccum = g.poff + 40;
-    }
-
-    // The rows of up to 32 neighbours colp[0 .. cnt32) into the entry buffer, as SpGen::stage_chunk does for sparse rows;
-    // a dense row is compacted to its non-zeros by the whole warp, row after row, while the rows fit.
-    __device__ __forceinline__ int stage(const int32_t *__restrict__ colp, int cnt32) {
-        const RowSrc &s = a->s;
-        if (s.hdr != nullptr) return g.stage_chunk(colp, cnt32);
-        const int lane = g.lane;
-        int total = 0, ne = 0;
-        if (lane == 0) g.poff[0] = 0;
-#pragma unroll 1
-        for (; ne < cnt32; ++ne) {
-            const double *row = s.F + (size_t)colp[ne] * s.ld;
-            int cv = 0;
-#pragma unroll 1
-            for (int c0 = 0; c0 < s.k; c0 += 32)
-                cv += __popc(__ballot_sync(0xffffffffu, c0 + lane < s.k && __ldg(row + c0 + lane) != 0.0));
-            if (total + cv > g.ecap) break;                 // (never for the first row: k <= ecap)
-#pragma unroll 1
-            for (int c0 = 0; c0 < s.k; c0 += 32) {
-                const int c = c0 + lane;
-                const double v = (c < s.k) ? __ldg(row + c) : 0.0;
-                const unsigned bal = __ballot_sync(0xffffffffu, v != 0.0);
-                if (v != 0.0) {
-                    const int p = total + __popc(bal & g.lt_mask);
-                    g.ent_val[p] = v;
-                    g.ent_idx[p] = (unsigned short)c;
-                }
-                total += __popc(bal);
-            }
-            if (lane == 0) g.poff[ne + 1] = (unsigned short)total;
-        }
-        __syncwarp();
-        return ne;
-    }
-
-    // PRE (:157-169) over the whole list, as SpGen::pre_range: returns S1 = sum_v edge terms and adds sum_v w_v F_v into
-    // g_d; the first call also marks the touched components.
-    __device__ __forceinline__ double pre(const int32_t *colp, int deg, bool first, int &nchunks, int &ne_last) {
-        const int lane = g.lane;
-        double S1 = 0.0;
-        nchunks = 0;
-        ne_last = 0;
-#pragma unroll 1
-        for (int cb = 0; cb < deg;) {
-            const int ne = stage(colp + cb, min(32, deg - cb));
-            double x = 0.0;
-            if (lane < ne) {
-                const int end = g.poff[lane + 1];
-#pragma unroll 1
-                for (int i = g.poff[lane]; i < end; ++i) x = fma(g.ent_val[i], g.fu_d[g.ent_idx[i]], x);
-            }
-            double w;
-            const double t = edge_term<true>(x, a->ec, w);
-            S1 += (lane < ne) ? t : 0.0;
-#pragma unroll 1
-            for (int e = 0; e < ne; ++e) {
-                const double we = __shfl_sync(0xffffffffu, w, e);
-                const int pe = g.poff[e], pn = g.poff[e + 1];
-#pragma unroll 1
-                for (int i = pe + lane; i < pn; i += 32) {
-                    const int c = g.ent_idx[i];
-                    g.g_d[c] = fma(we, g.ent_val[i], g.g_d[c]);
-                    if (first) atomicOr(tmask + (c >> 5), 1u << (c & 31));
-                }
-                __syncwarp();
-            }
-            cb += ne;
-            ne_last = ne;
-            ++nchunks;
-        }
-        return warp_sum(S1);
-    }
-
-    // tmask -> tl (ascending), nt
-    __device__ __forceinline__ void list_touched() {
-        const int lane = g.lane, W = g.ldp >> 5;
-        nt = 0;
-#pragma unroll 1
-        for (int w0 = 0; w0 < W; w0 += 32) {
-            const int w = w0 + lane;
-            unsigned bits = (w < W) ? tmask[w] : 0u;
-            const int pc = __popc(bits);
-            int incl = pc;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += t;
-            }
-            int p = nt + incl - pc;
-            while (bits) {
-                tl[p++] = (unsigned short)(32 * w + __ffs(bits) - 1);
-                bits &= bits - 1u;
-            }
-            nt += __shfl_sync(0xffffffffu, incl, 31);
-        }
-        __syncwarp();
-    }
-
-    // g_d (sum of weighted neighbour rows) -> gradient on the touched components; returns |g|^2 over all k components,
-    // lists the active ones (f > 0 or g > 0) in aidx and tells whether a candidate can reach max_f.
-    __device__ __forceinline__ double scan(int &m, bool &need_hi) {
-        const int lane = g.lane;
-        double G2 = 0.0, SF2 = 0.0;
-        bool hi_lane = false;
-        m = 0;
-#pragma unroll 1
-        for (int t0 = 0; t0 < nt; t0 += 32) {
-            const int t = t0 + lane;
-            const bool ok = t < nt;
-            const int c = ok ? (int)tl[t] : 0;
-            double f = 0.0, gr = 0.0;
-            if (ok) {
-                const double sf = __ldg(a->sumF + c);
-                f = g.fu_d[c];
-                gr = (g.g_d[c] - (sf + f)) + f;
-                g.g_d[c] = gr;
-                G2 = fma(gr, gr, G2);
-                SF2 = fma(sf, sf, SF2);
-            }
-            const bool act = ok && (f > 0.0 || gr > 0.0);
-            const unsigned bal = __ballot_sync(0xffffffffu, act);
-            if (act) {
-                g.aidx[m + __popc(bal & g.lt_mask)] = (unsigned short)c;
-                hi_lane |= (f + gr > a->max_f);
-            }
-            m += __popc(bal);
-        }
-        G2 = warp_sum(G2);
-        SF2 = warp_sum(SF2);
-        need_hi = __any_sync(0xffffffffu, hi_lane);
-        __syncwarp();
-        return (a->S2_all - SF2) + G2;
-    }
-
-    // Line search over the whole list (SpGen::ls_range with this staging): lane (j, h) returns its edges' share of the
-    // clamped edge terms of candidate s; `staged`: rows of a single chunk still staged from PRE.
-    __device__ __forceinline__ double ls(const int32_t *colp, int deg, double s, bool need_hi, int staged) {
-        const int lane = g.lane, h = lane >> 4;
-        const double max_f = a->max_f;
-        double sumterms = 0.0;
-#pragma unroll 1
-        for (int cb = 0; cb < deg;) {
-            const int ne = (staged > 0) ? staged : stage(colp + cb, min(32, deg - cb));
-            g.compact_active(ne);
-#pragma unroll 1
-            for (int e2 = 0; e2 < ne; e2 += 4) {
-                const int eA = e2 + h, eB = e2 + 2 + h;
-                const bool vA = eA < ne, vB = eB < ne;
-                const int iA = vA ? (int)g.poff[eA] : 0, nA = vA ? (int)g.poff[eA + 1] - iA : 0;
-                const int iB = vB ? (int)g.poff[eB] : 0, nB = vB ? (int)g.poff[eB + 1] - iB : 0;
-                const int nmax = max(nA, nB);
-                double DA = 0.0, DB = 0.0;
-#pragma unroll 1
-                for (int k = 0; k < nmax; ++k) {
-                    const bool ka = k < nA, kb = k < nB;
-                    const int ca = ka ? (int)g.ent_idx[iA + k] : 0, cb2 = kb ? (int)g.ent_idx[iB + k] : 0;
-                    const double pa = ka ? g.ent_val[iA + k] : 0.0, pb = kb ? g.ent_val[iB + k] : 0.0;
-                    const double fa = g.fu_d[ca], ga = g.g_d[ca], fb = g.fu_d[cb2], gb = g.g_d[cb2];
-                    if (need_hi) {
-                        DA = fma(clamp_step0(fa, s, ga, max_f), pa, DA);
-                        DB = fma(clamp_step0(fb, s, gb, max_f), pb, DB);
-                    } else {
-                        DA = fma(clamp_step0_lo(fa, s, ga), pa, DA);
-                        DB = fma(clamp_step0_lo(fb, s, gb), pb, DB);
-                    }
-                }
-                double tA, tB;
-                edge_term2(DA, DB, a->ec, tA, tB);
-                sumterms += vA ? tA : 0.0;
-                sumterms += vB ? tB : 0.0;
-            }
-            __syncwarp();
-            cb += ne;
-            staged = 0;
-        }
-        return sumterms;
-    }
-
-    // Armijo decision for the candidates tg .. tg+15 (SpGen::decide with sumF' = sumF + f).
-    __device__ __forceinline__ int decide(int tg, double s, bool jok, double sumterms, int m, bool need_hi, double llh_u, double G2) {
-        const int lane = g.lane, h = lane >> 4;
-        const double max_f = a->max_f;
-        double oa = 0.0, ob = 0.0;
-#pragma unroll 1
-        for (int t = h; t < m; t += 2) {
-            const int c = g.aidx[t];
-            const double f = g.fu_d[c], gr = g.g_d[c];
-            const double nf = need_hi ? clamp_step0(f, s, gr, max_f) : clamp_step0_lo(f, s, gr);
-            const double sf = ((__ldg(a->sumF + c) + f) - f) + nf;
-            oa = fma(nf, sf, oa);
-            ob = fma(nf, nf, ob);
-        }
-        oa += __shfl_xor_sync(0xffffffffu, oa, 16);
-        ob += __shfl_xor_sync(0xffffffffu, ob, 16);
-        const double result = (sumterms - oa) + ob;
-        const double rhs = llh_u + (a->alpha * s) * G2;
-        const unsigned pass = __ballot_sync(0xffffffffu, jok && (result >= rhs)) & 0xffffu;
-        return pass ? tg + __ffs(pass) - 1 : -1;          // lowest j == largest step (:182 max)
     }
 
     // Query node i, start to finish.  Leaves fu_d, g_d and tmask at zero.
@@ -1659,21 +1551,21 @@ struct FoldGen {
         const int64_t e0 = a->rowptr[i];
         const int deg = (int)(a->rowptr[i + 1] - e0);
         const int32_t *colp = a->col + e0;
+        const int nsteps = g.a->nsteps;
         double l = 0.0, lprev = 0.0;
-        int it = 0;
-        nt = 0;
+        int it = 0, nt = 0;
 #pragma unroll 1
         while (deg > 0) {
             // ---------------- PRE of f_it: l_it and the weighted neighbour sum ----------------
             int nchunks, ne_last;
-            const double S1 = pre(colp, deg, it == 0, nchunks, ne_last);
-            if (it == 0) list_touched();
+            const double S1 = warp_sum(g.pre_range(colp, 0, deg, true, nchunks, ne_last, it == 0));
+            if (it == 0) nt = g.list_touched(tl);
             double fusf = 0.0, fufu = 0.0;
 #pragma unroll 1
             for (int t = lane; t < nt; t += 32) {
                 const int c = tl[t];
                 const double f = g.fu_d[c];
-                fusf = fma(f, __ldg(a->sumF + c) + f, fusf);
+                fusf = fma(f, __ldg(g.s_sumF + c) + f, fusf);
                 fufu = fma(f, f, fufu);
             }
             l = (S1 - warp_sum(fusf)) + warp_sum(fufu);
@@ -1682,23 +1574,23 @@ struct FoldGen {
             int jstar = -1, m = 0;
             if (go) {
                 bool need_hi;
-                const double G2 = scan(m, need_hi);
+                const double G2 = g.scan_list(tl, nt, m, need_hi);
 #pragma unroll 1
-                for (int tg = 0; tg < a->nsteps && jstar < 0; tg += 16) {
+                for (int tg = 0; tg < nsteps && jstar < 0; tg += 16) {
                     const int j = tg + (lane & 15);
-                    const bool jok = j < a->nsteps;
-                    const double s = a->steps[jok ? j : 0];
-                    double st = ls(colp, deg, s, need_hi, (nchunks == 1 && tg == 0) ? ne_last : 0);
+                    const bool jok = j < nsteps;
+                    const double s = g.s_steps[jok ? j : 0];
+                    double st = g.ls_range(colp, 0, deg, s, need_hi, (nchunks == 1 && tg == 0) ? ne_last : 0);
                     st += __shfl_xor_sync(0xffffffffu, st, 16);
-                    jstar = decide(tg, s, jok, st, m, need_hi, l, G2);
+                    jstar = g.decide(tg, s, jok, st, m, need_hi, l, G2);
                 }
             }
             if (jstar >= 0) {                              // f_{it+1}: the accepted candidate, in place (one lane per component)
-                const double s = a->steps[jstar];
+                const double s = g.s_steps[jstar];
 #pragma unroll 1
                 for (int t = lane; t < m; t += 32) {
                     const int c = g.aidx[t];
-                    g.fu_d[c] = clamp_step0(g.fu_d[c], s, g.g_d[c], a->max_f);
+                    g.fu_d[c] = clamp_step0(g.fu_d[c], s, g.g_d[c], g.a->max_f);
                 }
                 __syncwarp();                              // (every lane is done reading g_d)
             }
@@ -1733,30 +1625,38 @@ struct FoldGen {
 #pragma unroll 1
         for (int t = lane; t < nt; t += 32) g.fu_d[tl[t]] = 0.0;
 #pragma unroll 1
-        for (int w = lane; w < (g.ldp >> 5); w += 32) tmask[w] = 0u;
+        for (int w = lane; w < (g.ldp >> 5); w += 32) g.tmask[w] = 0u;
         __syncwarp();
     }
 };
 
-// Grid-stride over the batch's query nodes, one warp each.  kWide: the per-warp vectors live in FoldArgs::scratch.
+// Grid-stride over the batch's query nodes, one warp each.  a: the context's step arguments (fill_args).  kWide: the
+// per-warp vectors live in FoldArgs::scratch.
 template <bool kWide>
-__global__ void fold_in_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ SparseArgs sp) {
+__global__ void fold_in_kernel(const __grid_constant__ StepArgs a, const __grid_constant__ FoldArgs fa, const __grid_constant__ SparseArgs sp) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int64_t gw = (int64_t)blockIdx.x * kFoldWarps + wib, nw = (int64_t)gridDim.x * kFoldWarps;
-    const size_t wb = fold_warp_bytes(a.s.ld);
-    unsigned char *base = kWide ? a.scratch + (size_t)gw * wb : smem_raw + (size_t)wib * wb;
+    const size_t wb = fold_warp_bytes(a.ld);
+    unsigned char *base = kWide ? fa.scratch + (size_t)gw * wb : smem_raw + (size_t)wib * wb;
     FoldGen<kWide> fg;
-    fg.carve(base, &sp, &a, lane);
+    fg.a = &fa;
+    fg.g.a = &a;
+    fg.g.sp = &sp;
+    fg.g.rs = &fa.s;
+    fg.g.s_steps = a.steps;
+    fg.g.s_sumF = a.sumF;
+    fg.g.S2_all = fa.S2_all;
+    fg.g.ec = {a.x_lo, a.x_hi, a.t_lo, a.t_hi, a.w_lo, a.w_hi};
+    fg.carve(base, a.ld, lane);
     if constexpr (!kWide) {
+        fg.g.clear_dense();
 #pragma unroll 1
-        for (int c = lane; c < fg.g.ldp; c += 32) { fg.g.fu_d[c] = 0.0; fg.g.g_d[c] = 0.0; }
-#pragma unroll 1
-        for (int w = lane; w < (fg.g.ldp >> 5); w += 32) fg.tmask[w] = 0u;
+        for (int w = lane; w < (fg.g.ldp >> 5); w += 32) fg.g.tmask[w] = 0u;
         __syncwarp();
     }
 #pragma unroll 1
-    for (int64_t i = gw; i < a.nq; i += nw) fg.node(i);
+    for (int64_t i = gw; i < fa.nq; i += nw) fg.node(i);
 }
 
 // An upper bound of the row length of each query node: min(k, the non-zeros of its neighbours' rows), one warp per node.
