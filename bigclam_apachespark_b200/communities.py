@@ -37,6 +37,25 @@ def extract(solver, delta: float):
     return comms, np.array(cids), member
 
 
+def group(comptr, members, zero_rows, zero_rows_everywhere: bool = True):
+    """BigClam.extract_communities()'s CSR as (communities: list of int32 arrays, community ids), the form extract()
+    returns: non-empty communities only, each ascending.  zero_rows_everywhere=True merges the all-zero rows into every
+    community, as coded; False leaves them out."""
+    comptr = np.asarray(comptr, dtype=np.int64)
+    members = np.asarray(members, dtype=np.int32)
+    zero_rows = np.asarray(zero_rows, dtype=np.int32)
+    merge = zero_rows_everywhere and len(zero_rows) > 0
+    comms, cids = [], []
+    for c in range(len(comptr) - 1):
+        idx = members[comptr[c]:comptr[c + 1]]
+        if merge:
+            idx = np.union1d(idx, zero_rows).astype(np.int32)
+        if len(idx):
+            comms.append(idx)
+            cids.append(c)
+    return comms, np.array(cids)
+
+
 def load_ground_truth(name: str = "com-amazon.cmty"):
     """Ground-truth communities fixture (dense vertex indices), written by tests/golden/make_fixtures.py."""
     z = np.load(os.path.join(FIXTURE_DIR, name + ".npz"))

@@ -1698,31 +1698,6 @@ extern "C" int bigclam_set_owned_nodes(bigclam_ctx *ctx, const int32_t *nodes, i
     return rebuild_order_list(ctx, rp, order);
 }
 
-// Community extraction on the current F (Bigclamv2.scala:223-230); see extract_kernel.
-extern "C" int bigclam_extract(bigclam_ctx *ctx, double delta, uint8_t *member_out /* n x k */, double *fmax_out /* n, optional */) {
-    if (ctx == nullptr) return BIGCLAM_EINVAL;
-    if (member_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "bigclam_extract: member_out is NULL");
-    CU(cudaSetDevice(ctx->device));
-    if (int re = ensure_dense(ctx)) return re;
-    const int k = ctx->p.k;
-    uint8_t *d_member = nullptr;
-    double *d_fmax = nullptr;
-    cudaError_t e = cudaMalloc(&d_member, (size_t)ctx->n * k);
-    if (e == cudaSuccess) e = cudaMalloc(&d_fmax, sizeof(double) * (size_t)ctx->n);
-    const int wpb = 8;
-    if (e == cudaSuccess) {
-        extract_kernel<<<(unsigned)((ctx->n + wpb - 1) / wpb), wpb * 32, 0, ctx->stream>>>(ctx->d_F[ctx->cur], ctx->n, k, ctx->ld, delta, d_member, d_fmax);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(member_out, d_member, (size_t)ctx->n * k, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess && fmax_out != nullptr) e = cudaMemcpyAsync(fmax_out, d_fmax, sizeof(double) * (size_t)ctx->n, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_member);
-    cudaFree(d_fmax);
-    if (e != cudaSuccess) return fail(ctx, BIGCLAM_ECUDA, "bigclam_extract: %s", cudaGetErrorString(e));
-    return BIGCLAM_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
 // Edge probabilities and link recommendations (bigclam_sparse.cuh, pair_x): read the current F where it lives (the
 // sparse rows, or the dense buffer of a dense context) on the context's stream.  They change no state: a speculative
@@ -1917,7 +1892,7 @@ static int sample_count(bigclam_ctx *ctx, uint64_t seed, double eps, SamplePlan 
     DevBuf<int64_t> deg;
     CU(ccnt.reserve((size_t)k));
     CU(cudaMemsetAsync(ccnt.p, 0, sizeof(unsigned int) * (size_t)k, ctx->stream));
-    colidx_kernel<false><<<grid_n, 32 * wpb, 0, ctx->stream>>>(s, n, ccnt.p, nullptr, nullptr);
+    colidx_kernel<false, NonZeroPred><<<grid_n, 32 * wpb, 0, ctx->stream>>>(s, n, NonZeroPred{}, 0, k, ccnt.p, nullptr, nullptr);
     CU(cudaGetLastError());
     std::vector<unsigned int> hcnt((size_t)k);
     CU(cudaMemcpyAsync(hcnt.data(), ccnt.p, sizeof(unsigned int) * (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1930,9 +1905,9 @@ static int sample_count(bigclam_ctx *ctx, uint64_t seed, double eps, SamplePlan 
     CU(cpos.reserve((size_t)k));
     CU(cudaMemcpyAsync(pl.colptr.p, hptr.data(), sizeof(int64_t) * ((size_t)k + 1), cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(cpos.p, hpos.data(), sizeof(unsigned long long) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
-    colidx_kernel<true><<<grid_n, 32 * wpb, 0, ctx->stream>>>(s, n, nullptr, cpos.p, pl.members.p);
+    colidx_kernel<true, NonZeroPred><<<grid_n, 32 * wpb, 0, ctx->stream>>>(s, n, NonZeroPred{}, 0, k, nullptr, cpos.p, pl.members.p);
     CU(cudaGetLastError());
-    colidx_sort_kernel<<<(unsigned)((k + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(pl.colptr.p, k, pl.members.p);
+    colidx_sort_kernel<<<(unsigned)((k + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(pl.colptr.p, k, 0, pl.members.p);
     CU(cudaGetLastError());
     pl.a = SampleArgs{s, pair_const(ctx), pl.colptr.p, pl.members.p, n, seed, eps};
     CU(deg.reserve((size_t)n));
@@ -2176,6 +2151,146 @@ extern "C" int bigclam_fold_in(bigclam_ctx *ctx, int64_t q, const int64_t *rowpt
     if (int rc = fold_args_check(ctx, what, q, rowptr, col, max_iter, rel_tol, indptr_out, indices_out, values_out)) return rc;
     if (q == 0) return BIGCLAM_OK;
     return fold_in(ctx, what, q, rowptr, col, max_iter, rel_tol, true, nullptr, indptr_out, indices_out, values_out, llh_out, iters_out);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Community extraction on the current F (Bigclamv2.scala:223-230; bigclam_sparse.cuh, is_member).  Reads F only, on
+// the context's stream, like the calls above.
+
+// Scratch bound of the extraction calls: query_budget, or BIGCLAM_EXTRACT_BUDGET bytes (tests: many ranges or batches).
+static cudaError_t extract_budget(int64_t &budget) {
+    const cudaError_t e = query_budget(budget);
+    if (const char *v = std::getenv("BIGCLAM_EXTRACT_BUDGET")) budget = std::max<int64_t>(1, std::atoll(v));
+    return e;
+}
+
+// member_out[u k + c] and fmax_out[u] for batches of rows whose n_b x k bytes stay within the scratch bound.
+extern "C" int bigclam_extract(bigclam_ctx *ctx, double delta, uint8_t *member_out /* n x k */, double *fmax_out /* n, optional */) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_extract";
+    if (member_out == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: member_out is NULL", what);
+    CU(cudaSetDevice(ctx->device));
+    const int64_t n = ctx->n, k = ctx->p.k;
+    if (n == 0) return BIGCLAM_OK;
+    const RowSrc s = row_src(ctx);
+    int64_t budget;
+    CU(extract_budget(budget));
+    const int64_t rows = std::max<int64_t>(1, std::min<int64_t>(n, budget / (k + 8)));
+    DevBuf<uint8_t> dm;
+    DevBuf<double> df;
+    if (dm.reserve((size_t)(rows * k)) != cudaSuccess || df.reserve((size_t)rows) != cudaSuccess)
+        return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte batch of rows", what, (long long)(rows * (k + 8)));
+    const int wpb = 8;
+    for (int64_t r0 = 0; r0 < n; r0 += rows) {
+        const int64_t r1 = std::min(n, r0 + rows);
+        extract_rows_kernel<<<(unsigned)((r1 - r0 + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(s, r0, r1, delta, dm.p, df.p);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(member_out + r0 * k, dm.p, (size_t)((r1 - r0) * k), cudaMemcpyDeviceToHost, ctx->stream));
+        if (fmax_out != nullptr) CU(cudaMemcpyAsync(fmax_out + r0, df.p, sizeof(double) * (size_t)(r1 - r0), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    return BIGCLAM_OK;
+}
+
+static int extract_args_check(bigclam_ctx *ctx, const char *what, double delta, const void *out1, const void *out2, const void *out3) {
+    if (!(delta > 0.0)) return fail(ctx, BIGCLAM_EINVAL, "%s: delta = %g, must be > 0", what, delta);
+    if (out1 == nullptr || out2 == nullptr || out3 == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: NULL output", what);
+    return BIGCLAM_OK;
+}
+
+// The count pass: ptr (host, k + 2 entries) = the exclusive scan of the column sizes, column k being the zero rows.
+static int extract_count(bigclam_ctx *ctx, const char *what, double delta, std::vector<int64_t> &ptr) {
+    CU(cudaSetDevice(ctx->device));
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k;
+    ptr.assign((size_t)k + 2, 0);
+    if (n == 0) return BIGCLAM_OK;
+    const int wpb = 4;
+    DevBuf<unsigned int> ccnt;
+    DevBuf<unsigned long long> neg;
+    CU(ccnt.reserve((size_t)k + 1));
+    CU(neg.reserve(1));
+    CU(cudaMemsetAsync(ccnt.p, 0, sizeof(unsigned int) * ((size_t)k + 1), ctx->stream));
+    CU(cudaMemsetAsync(neg.p, 0xff, sizeof(unsigned long long), ctx->stream));
+    colidx_kernel<false, MemberPred><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(row_src(ctx), n, MemberPred{delta, k, neg.p}, 0, k + 1,
+                                                                                        ccnt.p, nullptr, nullptr);
+    CU(cudaGetLastError());
+    std::vector<unsigned int> hcnt((size_t)k + 1);
+    unsigned long long hneg = 0;
+    CU(cudaMemcpyAsync(hcnt.data(), ccnt.p, sizeof(unsigned int) * ((size_t)k + 1), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&hneg, neg.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (hneg != ~0ull) return fail(ctx, BIGCLAM_EUNSUPPORTED, "%s: row %llu has a negative entry (F must be >= 0)", what, hneg);
+    for (int32_t c = 0; c <= k; ++c) ptr[(size_t)c + 1] = ptr[(size_t)c] + hcnt[(size_t)c];
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_extract_nnz(bigclam_ctx *ctx, double delta, int64_t *nnz_out, int64_t *n_zero_rows_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_extract_nnz";
+    if (int rc = extract_args_check(ctx, what, delta, nnz_out, n_zero_rows_out, nnz_out)) return rc;
+    std::vector<int64_t> ptr;
+    if (int rc = extract_count(ctx, what, delta, ptr)) return rc;
+    const int32_t k = ctx->p.k;
+    *nnz_out = ptr[(size_t)k];
+    *n_zero_rows_out = ptr[(size_t)k + 1] - ptr[(size_t)k];
+    return BIGCLAM_OK;
+}
+
+// Count, then the columns 0 .. k (k = the zero rows) in consecutive ranges whose lists fit the scratch bound (a longer
+// list gets a range of its own): fill, sort, copy out.
+extern "C" int bigclam_extract_grouped(bigclam_ctx *ctx, double delta, int64_t *comptr_out, int32_t *members_out, int32_t *zero_rows_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_extract_grouped";
+    if (int rc = extract_args_check(ctx, what, delta, comptr_out, members_out, zero_rows_out)) return rc;
+    std::vector<int64_t> ptr;
+    if (int rc = extract_count(ctx, what, delta, ptr)) return rc;
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k;
+    std::copy(ptr.begin(), ptr.begin() + k + 1, comptr_out);
+    if (ptr[(size_t)k + 1] == 0) return BIGCLAM_OK;
+    int64_t budget;
+    CU(extract_budget(budget));
+    const int64_t budget_entries = std::max<int64_t>(1, budget / (int64_t)sizeof(int32_t));
+    const RowSrc s = row_src(ctx);
+    DevBuf<int64_t> dptr;
+    DevBuf<unsigned long long> cpos;
+    DevBuf<int32_t> dout;
+    CU(dptr.reserve((size_t)k + 2));
+    CU(cudaMemcpyAsync(dptr.p, ptr.data(), sizeof(int64_t) * ((size_t)k + 2), cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<unsigned long long> hpos;
+    const int wpb = 4;
+    for (int32_t c0 = 0; c0 <= k;) {
+        int32_t c1 = c0 + 1;
+        while (c1 <= k && ptr[(size_t)c1 + 1] - ptr[(size_t)c0] <= budget_entries) ++c1;
+        const int64_t base = ptr[(size_t)c0], total = ptr[(size_t)c1] - base;
+        if (total > 0) {
+            if (dout.reserve((size_t)total) != cudaSuccess) {
+                if (c1 - c0 == 1 && c0 == k)
+                    return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for the %lld zero rows", what, (long long)total);
+                if (c1 - c0 == 1)
+                    return fail(ctx, BIGCLAM_ENOMEM, "%s: community %d has %lld members; no room for them", what, c0, (long long)total);
+                return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte range of communities %d..%d", what,
+                            (long long)(total * (int64_t)sizeof(int32_t)), c0, c1 - 1);
+            }
+            hpos.resize((size_t)(c1 - c0));
+            for (int32_t c = c0; c < c1; ++c) hpos[(size_t)(c - c0)] = (unsigned long long)(ptr[(size_t)c] - base);
+            CU(cpos.reserve((size_t)(c1 - c0)));
+            CU(cudaMemcpyAsync(cpos.p, hpos.data(), sizeof(unsigned long long) * (size_t)(c1 - c0), cudaMemcpyHostToDevice, ctx->stream));
+            colidx_kernel<true, MemberPred><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(s, n, MemberPred{delta, k, nullptr}, c0, c1,
+                                                                                                nullptr, cpos.p, dout.p);
+            CU(cudaGetLastError());
+            colidx_sort_kernel<<<(unsigned)((c1 - c0 + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(dptr.p + c0, c1 - c0, base, dout.p);
+            CU(cudaGetLastError());
+            const int64_t nm = std::max<int64_t>(0, std::min(ptr[(size_t)k], ptr[(size_t)c1]) - base);   // entries of communities < k
+            if (nm > 0) CU(cudaMemcpyAsync(members_out + base, dout.p, sizeof(int32_t) * (size_t)nm, cudaMemcpyDeviceToHost, ctx->stream));
+            if (total > nm)
+                CU(cudaMemcpyAsync(zero_rows_out, dout.p + nm, sizeof(int32_t) * (size_t)(total - nm), cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaStreamSynchronize(ctx->stream));           // (hpos is reused by the next range)
+        }
+        c0 = c1;
+    }
+    return BIGCLAM_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2440,6 +2555,16 @@ extern "C" int bigclam_multi_fold_in(bigclam_multi *m, int64_t q, const int64_t 
                                      int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     MCALL(bigclam_fold_in(m->r[0], q, rowptr, col, max_iter, rel_tol, indptr_out, indices_out, values_out, llh_out, iters_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_extract_nnz(bigclam_multi *m, double delta, int64_t *nnz_out, int64_t *n_zero_rows_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_extract_nnz(m->r[0], delta, nnz_out, n_zero_rows_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_extract_grouped(bigclam_multi *m, double delta, int64_t *comptr_out, int32_t *members_out, int32_t *zero_rows_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_extract_grouped(m->r[0], delta, comptr_out, members_out, zero_rows_out), m->r[0]);
     return BIGCLAM_OK;
 }
 

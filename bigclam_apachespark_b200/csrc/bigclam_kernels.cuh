@@ -1376,24 +1376,4 @@ __global__ void colsum_final_kernel(const double *part, int nchunks, int ld, dou
     out[col] = v;
 }
 
-// Community extraction, Bigclamv2.scala:223-230: node u belongs to community c iff F_uc >= delta; a node whose
-// largest entry is below delta belongs to the communities where F_uc equals that maximum (ties included,
-// `value == Fmax` at :227).  One warp per node; member is n x k bytes (0/1), fmax the row maximum.
-__global__ void extract_kernel(const double *F, int64_t n, int k, int ld, double delta, uint8_t *member, double *fmax) {
-    const int lane = threadIdx.x & 31;
-    const int64_t u = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (u >= n) return;
-    const double *row = F + (size_t)u * ld;
-    double mx = -1.0;
-    for (int c = lane; c < k; c += 32) mx = fmax2(mx, row[c]);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmax2(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    const bool below = mx < delta;
-    for (int c = lane; c < k; c += 32) {
-        const double v = row[c];
-        member[(size_t)u * k + c] = below ? (v == mx) : (v >= delta);
-    }
-    if (lane == 0) fmax[u] = mx;
-}
-
 }  // namespace bigclam

@@ -1379,33 +1379,130 @@ __device__ __forceinline__ double pair_x_first(const RowSrc &s, int64_t u, int64
     return x;
 }
 
-// Column index of the current rows: colptr[k + 1] and members, M_c = members[colptr[c], colptr[c + 1]) ascending.
-// Built by count, scan (host) and fill, one warp per row; the fill takes slots in any order and the sort makes the
-// lists ascending, so the index is the same from run to run.
-template <bool kFill>
-__global__ void colidx_kernel(RowSrc s, int64_t n, unsigned int *__restrict__ colcnt, unsigned long long *__restrict__ colpos,
-                              int32_t *__restrict__ members) {
+// Row u as stored: cnt entries vals[0, cnt) at components idx[i] (sparse rows) or i (dense rows, cnt = k).  The k - cnt
+// components a sparse row does not store are zeros.
+struct RowView {
+    const double *vals;
+    const unsigned short *idx;         // nullptr: dense row
+    int cnt;
+};
+__device__ __forceinline__ RowView row_view(const RowSrc &s, int64_t u) {
+    if (s.hdr == nullptr) return RowView{s.F + (size_t)u * s.ld, nullptr, s.k};
+    const uint64_t hu = s.hdr[u];
+    const double *vals = s.pool + sp_off8(hu);
+    return RowView{vals, sp_idx(vals, sp_cnt(hu)), (int)sp_cnt(hu)};
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Community membership, Bigclamv2.scala:225-228 (bigclam_extract, bigclam_extract_grouped).  With fmax_u the maximum of
+// row u over all k components (the zeros a sparse row does not store included), u is a member of community c iff
+//   fmax_u <  delta:  F_uc == fmax_u   (ties included, `value == Fmax` at :227)
+//   fmax_u >= delta:  F_uc >= delta.
+// row_fmax is warp-uniform; every lane gets the same bits whatever the layout.
+__device__ __forceinline__ double row_fmax(const RowSrc &s, const RowView &r, int lane) {
+    double mx = r.cnt < s.k ? 0.0 : -INFINITY;
+    for (int i = lane; i < r.cnt; i += 32) mx = fmax2(mx, r.vals[i]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmax2(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    return mx;
+}
+__host__ __device__ __forceinline__ bool is_member(double v, double fmax, double delta) { return fmax < delta ? v == fmax : v >= delta; }
+
+#ifdef BIGCLAM_EMU          // host emulation (tests/emu): no atomicMin there
+inline void atomic_min_u64(unsigned long long *p, unsigned long long v) {
+    unsigned long long old = __atomic_load_n(p, __ATOMIC_SEQ_CST);
+    while (v < old && !__atomic_compare_exchange_n(p, &old, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {
+    }
+}
+#else
+__device__ __forceinline__ void atomic_min_u64(unsigned long long *p, unsigned long long v) { atomicMin(p, v); }
+#endif
+
+// Which entries of a row the column index lists (colidx_kernel's predicate).  row() runs once per row with the whole
+// warp and gives the row's state; take(state, v) says whether an entry v != 0 is listed; whole(state) names a column
+// that takes the row itself (-1: none).
+struct NonZeroPred {               // every non-zero (the sampler's M_c)
+    struct Row {};
+    __device__ __forceinline__ Row row(const RowSrc &, const RowView &, int64_t, int) const { return Row{}; }
+    __device__ __forceinline__ bool take(const Row &, double) const { return true; }
+    __device__ __forceinline__ int whole(const Row &) const { return -1; }
+};
+// Membership for delta > 0 and F >= 0 (bigclam_extract_grouped): a row with a non-zero entry has its members among its
+// non-zeros; an all-zero row (fmax = 0 < delta) is a member of every community and goes, once, to column k.  neg (count
+// pass only) takes the smallest row with a negative entry, for which the rule above does not hold.
+struct MemberPred {
+    double delta;
+    int k;
+    unsigned long long *neg;
+    struct Row {
+        double fmax;
+    };
+    __device__ __forceinline__ Row row(const RowSrc &s, const RowView &r, int64_t u, int lane) const {
+        if (neg != nullptr) {
+            bool any = false;
+            for (int i = lane; i < r.cnt; i += 32) any |= r.vals[i] < 0.0;
+            if (any) atomic_min_u64(neg, (unsigned long long)u);
+        }
+        return Row{row_fmax(s, r, lane)};
+    }
+    __device__ __forceinline__ bool take(const Row &st, double v) const { return is_member(v, st.fmax, delta); }
+    __device__ __forceinline__ int whole(const Row &st) const { return st.fmax == 0.0 ? k : -1; }
+};
+
+// Column index of the current rows under a predicate P: colptr and members, list c = members[colptr[c], colptr[c + 1])
+// ascending.  Built by count, scan (host) and fill, one warp per row; the fill takes slots in any order and the sort
+// makes the lists ascending, so the index is the same from run to run.  Only the columns [c0, c1) are counted or
+// filled: count adds to colcnt[c], fill writes members[colpos[c - c0]++] (positions relative to the caller's buffer).
+template <bool kFill, class P>
+__global__ void colidx_kernel(RowSrc s, int64_t n, P pred, int32_t c0, int32_t c1, unsigned int *__restrict__ colcnt,
+                              unsigned long long *__restrict__ colpos, int32_t *__restrict__ members) {
     const int lane = threadIdx.x & 31;
     const int64_t u = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (u >= n) return;
-    const bool sparse = s.hdr != nullptr;
-    const uint64_t hu = sparse ? s.hdr[u] : 0;
-    const int cnt = sparse ? (int)sp_cnt(hu) : s.k;
-    const double *vals = sparse ? s.pool + sp_off8(hu) : s.F + (size_t)u * s.ld;
-    const unsigned short *idx = sparse ? sp_idx(vals, (uint32_t)cnt) : nullptr;
-    for (int i = lane; i < cnt; i += 32) {
-        if (vals[i] == 0.0) continue;
-        const int c = sparse ? (int)idx[i] : i;
-        if (kFill) members[atomicAdd(&colpos[c], 1ull)] = (int32_t)u;
+    const RowView r = row_view(s, u);
+    const typename P::Row st = pred.row(s, r, u, lane);
+    auto list = [&](int c) {
+        if (c < c0 || c >= c1) return;
+        if (kFill) members[atomicAdd(&colpos[c - c0], 1ull)] = (int32_t)u;
         else atomicAdd(&colcnt[c], 1u);
+    };
+    const int w = pred.whole(st);
+    if (w >= 0) {
+        if (lane == 0) list(w);
+        return;
+    }
+    for (int i = lane; i < r.cnt; i += 32) {
+        const double v = r.vals[i];
+        if (v == 0.0 || !pred.take(st, v)) continue;
+        list(r.idx != nullptr ? (int)r.idx[i] : i);
     }
 }
 
-__global__ void colidx_sort_kernel(const int64_t *__restrict__ colptr, int32_t k, int32_t *__restrict__ members) {
+// Sorts each list c < nc of members[colptr[c] - base, colptr[c + 1] - base), one warp per list.
+__global__ void colidx_sort_kernel(const int64_t *__restrict__ colptr, int32_t nc, int64_t base, int32_t *__restrict__ members) {
     const int lane = threadIdx.x & 31;
     const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (c >= k) return;
-    warp_sort_u32(reinterpret_cast<uint32_t *>(members + colptr[c]), colptr[c + 1] - colptr[c], lane);
+    if (c >= nc) return;
+    warp_sort_u32(reinterpret_cast<uint32_t *>(members + (colptr[c] - base)), colptr[c + 1] - colptr[c], lane);
+}
+
+// bigclam_extract's n x k bytes for the rows [r0, r1), one warp per row: member[(u - r0) k + c] = is_member(F_uc), and
+// fmax[u - r0] = row_fmax.  A sparse row writes its implicit zeros' verdict first, then its stored entries.
+__global__ void extract_rows_kernel(RowSrc s, int64_t r0, int64_t r1, double delta, uint8_t *__restrict__ member,
+                                    double *__restrict__ fmax) {
+    const int lane = threadIdx.x & 31;
+    const int64_t u = r0 + (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (u >= r1) return;
+    const RowView r = row_view(s, u);
+    const double mx = row_fmax(s, r, lane);
+    uint8_t *m = member + (size_t)(u - r0) * s.k;
+    if (r.idx != nullptr) {
+        const uint8_t z = is_member(0.0, mx, delta);
+        for (int c = lane; c < s.k; c += 32) m[c] = z;
+        __syncwarp();
+    }
+    for (int i = lane; i < r.cnt; i += 32) m[r.idx != nullptr ? (int)r.idx[i] : i] = is_member(r.vals[i], mx, delta);
+    if (lane == 0) fmax[u - r0] = mx;
 }
 
 struct SampleArgs {

@@ -447,6 +447,29 @@ class BigClam:
             check(lib.bigclam_fold_in(self._ctx, *args, *outs), self._ctx)
         return indptr, indices[:nnz.value], values[:nnz.value], llh, iters
 
+    def extract_communities(self, delta):
+        """The communities of Bigclamv2.scala:223-230 grouped by community, on the GPU, with no n x K image anywhere.
+        delta > 0 (not NaN; inf allowed) and F >= 0.  Returns (comptr int64[K + 1], members int32[nnz], zero_rows
+        int32[z]): community c is members[comptr[c]:comptr[c + 1]] ascending; an all-zero row is, as coded, a member of
+        every community and is listed once in zero_rows (ascending) instead.  communities.group() turns this into
+        communities.extract()'s lists."""
+        lib = _lib.load()
+        delta = float(delta)
+        nnz, z = C.c_int64(), C.c_int64()
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_extract_nnz(self._multi, delta, C.byref(nnz), C.byref(z)))
+        else:
+            check(lib.bigclam_extract_nnz(self._need(), delta, C.byref(nnz), C.byref(z)), self._ctx)
+        comptr = np.zeros(self.K + 1, dtype=np.int64)
+        members = np.empty(max(nnz.value, 1), dtype=np.int32)
+        zero_rows = np.empty(max(z.value, 1), dtype=np.int32)
+        outs = (comptr.ctypes.data, members.ctypes.data, zero_rows.ctypes.data)
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_extract_grouped(self._multi, delta, *outs))
+        else:
+            check(lib.bigclam_extract_grouped(self._ctx, delta, *outs), self._ctx)
+        return comptr, members[:nnz.value], zero_rows[:z.value]
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

@@ -273,9 +273,43 @@ void bigclam_graph_free(bigclam_graph *g);
  * member_out[u*k + c] = 1 iff F_uc >= delta, or, when the row maximum is below delta, iff F_uc equals the
  * row maximum (ties included, as coded at :227).  delta is computed by the caller:
  * sqrt(-log(1 - e)) with e = 2*count/(N*(N-1)) (:223-224; `count` there is the number of vertices that
- * have edges, not |E|).
+ * have edges, not |E|).  fmax_out (optional, n) gets the row maxima.
+ *
+ * Membership, the one definition of this call and bigclam_extract_grouped (:225-228): with fmax_u the maximum of row u
+ * over ALL k components (the zeros a sparse row does not store included), u is a member of community c iff
+ *   fmax_u <  delta:  F_uc == fmax_u   (ties included)
+ *   fmax_u >= delta:  F_uc >= delta.
+ * bigclam_extract reads the rows where they live (sparse or dense) in batches of rows whose n_b x k bytes stay within
+ * the smaller of 1 GiB and 10 % of the free device memory; no dense image of F is built.
  */
 int bigclam_extract(bigclam_ctx *ctx, double delta, uint8_t *member_out, double *fmax_out);
+
+/*
+ * The communities grouped by community (the flatMap / groupByKey of :229-230), without an n x k image anywhere.
+ * delta must be > 0 and not NaN (+inf is allowed: every row goes to its maximum entries), else BIGCLAM_EINVAL before
+ * any device work; with delta <= 0 every zero entry would be a membership.  F must have no negative entry (the step
+ * never leaves one, bigclam_set_F can): a row with one gives BIGCLAM_EUNSUPPORTED naming the smallest such row.  Then
+ * every row is one of two kinds:
+ *   all zero (fmax_u = 0 < delta): as coded a member of every community; listed ONCE, in zero_rows_out (ascending),
+ *                                  and left out of the per-community lists;
+ *   any other row:                 its memberships are among its non-zero entries.
+ * The output is a CSR over communities: comptr_out (k + 1, int64), members_out (nnz, int32, each community's nodes
+ * ascending, zero rows excluded), zero_rows_out (z, int32, ascending).  It depends on (F bits, delta) only: not on the
+ * row layout, the batch cut, the number of GPUs or the device.
+ *
+ * bigclam_extract_nnz gives nnz and z; bigclam_extract_grouped fills the three outputs (sized with them; it counts
+ * again, nothing is kept between the calls).  Both read F only, like the calls below: no state changes (F, sumF,
+ * accepted indices, a speculative step), the context's stream, synchronous.  A NULL output (also for nnz = 0 or z = 0)
+ * gives BIGCLAM_EINVAL.  The communities are filled in consecutive ranges whose members stay within the smaller of
+ * 1 GiB and 10 % of the free device memory (a longer community gets a range of its own); BIGCLAM_ENOMEM, naming the
+ * community, when even that cannot be allocated.
+ */
+int bigclam_extract_nnz(bigclam_ctx *ctx, double delta, int64_t *nnz_out, int64_t *n_zero_rows_out);
+int bigclam_extract_grouped(bigclam_ctx *ctx, double delta, int64_t *comptr_out /* k + 1 */, int32_t *members_out /* nnz */,
+                            int32_t *zero_rows_out /* z */);
+/* The same for a multi-GPU handle: rank 0's replica is read, errors go to bigclam_multi_last_error. */
+int bigclam_multi_extract_nnz(bigclam_multi *m, double delta, int64_t *nnz_out, int64_t *n_zero_rows_out);
+int bigclam_multi_extract_grouped(bigclam_multi *m, double delta, int64_t *comptr_out, int32_t *members_out, int32_t *zero_rows_out);
 
 /*
  * The fitted model as a model of edges (the clamp of bigclam4-7.scala:166, the edge term of :218), on the current F:

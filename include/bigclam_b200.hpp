@@ -15,7 +15,8 @@
 //   SGDFindC()                                        :225-243   SGDFindC()
 //   MBSGD()       bigclamv3-7.scala:206-222, Bigclamv2.scala:203-219   MBSGD(version)
 //   K sweep                                           :244-266   sweep_K()
-//   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta)
+//   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta),
+//                                                                extract_grouped(delta, ...)
 //   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m),
 //                                                                sample_graph(seed, eps)
 //   rows for new nodes, the fit held fixed (:157-184 per node)    fold_in(rowptr, col, max_iter, rel_tol, ...)
@@ -29,6 +30,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <iterator>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -200,22 +202,39 @@ public:
     // Community extraction as coded in Bigclamv2.scala:223-230.  delta_threshold: `e = 2.0*count/(N*(N-1)); sqrt(-log(1-e))`
     // (:223-224; in the script `count` is the number of vertices that have edges, the thesis uses |E|: pass what you mean).
     // extract(): communities[c] = vertices u with F_uc >= delta, or, when the row maximum is below delta, with F_uc equal to
-    // the row maximum (:227); the flatMap / groupByKey of :229-230 is the regrouping by community id done here.
+    // the row maximum (:227), ascending; an all-zero row is in every community, as coded.  The flatMap / groupByKey of
+    // :229-230 runs on the GPU (bigclam_extract_grouped: delta > 0, F >= 0).  Works for multi-GPU handles too.
     static double delta_threshold(int64_t n_vertices, int64_t count) {
         const double e = 2.0 * (double)count / ((double)n_vertices * ((double)n_vertices - 1.0));
         return std::sqrt(-std::log(1.0 - e));
     }
     std::vector<std::vector<int32_t>> extract(double delta) {
-        need();
-        if (multi_ != nullptr) throw Error(BIGCLAM_EUNSUPPORTED, "extract: single-GPU contexts only (read F() and regroup on the host)");
-        std::vector<uint8_t> member((size_t)(n_ * K_));
-        std::vector<double> fmax((size_t)n_);
-        check(bigclam_extract(ctx_, delta, member.data(), fmax.data()), "extract");
+        std::vector<int64_t> comptr;
+        std::vector<int32_t> members, zero_rows;
+        extract_grouped(delta, comptr, members, zero_rows);
         std::vector<std::vector<int32_t>> comms((size_t)K_);
-        for (int64_t u = 0; u < n_; ++u)
-            for (int c = 0; c < K_; ++c)
-                if (member[(size_t)(u * K_ + c)]) comms[(size_t)c].push_back((int32_t)u);
+        for (int c = 0; c < K_; ++c) {
+            auto &out = comms[(size_t)c];
+            out.reserve((size_t)(comptr[(size_t)c + 1] - comptr[(size_t)c]) + zero_rows.size());
+            std::merge(members.begin() + comptr[(size_t)c], members.begin() + comptr[(size_t)c + 1], zero_rows.begin(), zero_rows.end(),
+                       std::back_inserter(out));
+        }
         return comms;
+    }
+    // The same communities as a CSR over communities (bigclam_extract_grouped): community c is
+    // members[comptr[c] .. comptr[c + 1]) ascending, and the all-zero rows are listed once, ascending, in zero_rows.
+    void extract_grouped(double delta, std::vector<int64_t> &comptr, std::vector<int32_t> &members, std::vector<int32_t> &zero_rows) {
+        need();
+        int64_t nnz = 0, z = 0;
+        check(multi_ ? bigclam_multi_extract_nnz(multi_, delta, &nnz, &z) : bigclam_extract_nnz(ctx_, delta, &nnz, &z), "extract");
+        comptr.assign((size_t)K_ + 1, 0);
+        members.assign((size_t)std::max<int64_t>(nnz, 1), 0);
+        zero_rows.assign((size_t)std::max<int64_t>(z, 1), 0);
+        check(multi_ ? bigclam_multi_extract_grouped(multi_, delta, comptr.data(), members.data(), zero_rows.data())
+                     : bigclam_extract_grouped(ctx_, delta, comptr.data(), members.data(), zero_rows.data()),
+              "extract");
+        members.resize((size_t)nnz);
+        zero_rows.resize((size_t)z);
     }
 
     // The fitted model as a model of edges, P(u,v) = 1 - exp(-F_u.F_v) with the clamp of :166 (bigclam_pair_affinity):
