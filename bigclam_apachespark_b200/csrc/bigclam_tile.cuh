@@ -10,7 +10,7 @@
 //   PRE     lane = edge: x_e = fu . fv_e with fu looked up through the node's bitmask of non-zero components
 //           (rank = popcount below the bit), exp/log once for 32 edges of up to 8 nodes;
 //   slots   the components a node touches (its own and its neighbours' non-zeros) get consecutive slots in
-//           ascending component order (bitmask + prefix popcounts): slot s holds (fu_c, grad_c);
+//           ascending component order (bitmask + prefix popcounts): slot s holds grad_c and where fu_c is in the own row;
 //   axpy    lane groups of 32/nn lanes per node add w_e * fv_e into the slots, edge by edge (CSR order);
 //   bounds  which (node, trial) pairs can pass the Armijo test at all (phase H2: a concavity bound on the node's objective
 //           from the PRE quantities); on the bench workload 9 of 10 nodes have no such pair and keep their row;
@@ -59,10 +59,10 @@ constexpr int kTlMaxEdges = 32;
 #endif
 #define BIGCLAM_PRAGMA(x) _Pragma(#x)
 #define BIGCLAM_UNROLL(n) BIGCLAM_PRAGMA(unroll n)
-// one block of 15 warps per SM at K <= 256: the line-search entry lists overlay buffers that are dead by then (15.2 KB
-// per warp at K = 200, see tl_lsov_bytes), and the block's steps and sumF are held once per SM
+// one block of 18 warps per SM at K <= 256: buffers whose lifetimes do not overlap share bytes (12.2 KB per warp up to
+// K = 832, see the warp region below), and the block's steps and sumF are held once per SM
 #ifndef BIGCLAM_TL_WARPS
-#define BIGCLAM_TL_WARPS 15
+#define BIGCLAM_TL_WARPS 18
 #endif
 #ifndef BIGCLAM_TL_BLOCKS
 #define BIGCLAM_TL_BLOCKS 1
@@ -79,48 +79,56 @@ constexpr int kTlThreads = kTlWarps * 32;
 constexpr int kTlMbars = (kTlWarps + 1) & ~1;       // mbarrier slots: an even count keeps the warp regions 16-byte aligned
 constexpr int kTlWideWarps = 6;                      // warps per block of the wide variant (wide_step)
 static_assert(kTlStage16 >= 264, "the neighbour staging buffer doubles as xs[32 edges + 1 scratch row][16 trials]");
-static_assert(2 * kTlSlots >= 3 * kTlAct, "fg must hold (f, g) and sumF - f of the active components after compaction");
 static_assert(kTlEnt <= 256, "entry lists: edge ids are bytes");
 static_assert(kTlAct <= 255, "active-component ids of the entry lists are bytes");
-static_assert(16 * kTlSlots >= 24 * kTlAct + 2 * 16 * kTlMaxEdges, "fg also holds sumF - f of the active components and the pair list of a line-search round");
-// behind the pair list, fg also holds the entry-list counters and offsets of phase I (lcnt, loff)
-constexpr int kTlLcntOff = 24 * kTlAct + 2 * 16 * kTlMaxEdges;
-static_assert(16 * kTlSlots >= kTlLcntOff + 4 * kTlAct + 2 * (kTlAct + 2), "fg also holds lcnt and loff behind the pair list");
+static_assert(2 * kTlOwn16 < 255, "own-entry indices of the slots are bytes (0xff: not an own component)");
 
-// The entry lists of phases I-K overlay buffers that are dead by then:
-//   ent_val on stageO | we | tmask | pref_t  (stageO and tmask are last read in C2, pref_t in C2, we (as we2) in H2;
-//     at small K that span is shorter than ent_val, and the overlay takes the larger of the two);
-//   ent_e, ent_a on slot_c[kTlAct..kTlSlots)  (after the compaction in H, slot_c is read below A <= kTlAct - 1 only).
+// The warp region of the tile path.  Buffers whose lifetimes do not overlap share bytes (phases: TlWarp::run):
+//   stageN   neighbour rows  A-I                  | xs (edge x trial)  J-K
+//   gd       g per slot  E-H                      | g of the active components [kTlAct]  H-L, ent_val behind them  I-J
+//   stageO   own rows  A-H (fu of a slot is read through slot_o)  | we2  H2 | lcnt, loff  I | asfm  J
+//   slot_c   component of a slot  C2-L (below A only after H)     | ent_e, ent_a behind kTlAct  I-J
+//   slot_o   own-entry index of a slot (byte)  C2-H               | amap (slot -> active index, byte)  H-I   | plist  J
+//   erow, e_soff, e_cnt, e_io2 (entry -> row, rows' places)  A-I                                          | plist  J
+//   fa       fu of the active components [kTlAct]  H-L;  before: tmask | pref_t  A-C2, we  D-G
+// Everything but the tail (fa, or tmask | pref_t: 48 B per mask word of a node) is at a fixed offset.
+constexpr int kTlOffG = 16 * kTlStage16;
+constexpr int kTlOffOwn = kTlOffG + 8 * kTlSlots;
+constexpr int kTlOffLlh = kTlOffOwn + 16 * kTlOwn16;                  // n_llh, n_G2 [8 doubles each]
+constexpr int kTlOffSlotC = kTlOffLlh + 2 * 8 * 8;
+constexpr int kTlOffAmap = kTlOffSlotC + 2 * kTlSlots;
+constexpr int kTlOffErow = kTlOffAmap + kTlSlots;
+constexpr int kTlOffESoff = kTlOffErow + kTlErow;                     // e_soff, e_cnt [40 u16 each: 32 edges, then 8 nodes]
+constexpr int kTlOffEIo2 = kTlOffESoff + 2 * 2 * 40;
+constexpr int kTlOffEpos = kTlOffEIo2 + 2 * 32;
+constexpr int kTlOffENi = kTlOffEpos + 2 * 34;
+constexpr int kTlOffNu = (kTlOffENi + 32 + 3) & ~3;                   // n_u [8 int]
+constexpr int kTlOffNes = kTlOffNu + 4 * kTlMaxNodes;                 // n_es, n_sb, n_ab [12 u16 each], n_m [8], n_q [16], n_sv [8]
+constexpr int kTlOffNjs = kTlOffNes + 2 * (12 + 12 + 12 + 8 + 16 + 8); // n_js, n_want, n_sl [8 bytes each], n_cnt [2]
+constexpr int kTlOffFa = (kTlOffNjs + 3 * 8 + 2 + 7) & ~7;
+static_assert(8 * kTlAct + 8 * kTlEnt <= 8 * kTlSlots, "ent_val fits in gd behind the gradients of the active components");
+static_assert(16 * kTlOwn16 >= 4 * kTlAct + 2 * (kTlAct + 2) && 16 * kTlOwn16 >= 8 * kTlAct && 16 * kTlOwn16 >= 8 * 32,
+              "stageO holds lcnt | loff, then asfm, and we2");
+static_assert(kTlOffEIo2 + 2 * 32 - kTlOffAmap >= 2 * 16 * kTlMaxEdges, "the pair list of a line-search round fits on amap .. e_io2");
 static_assert(kTlSlots - kTlAct >= kTlEnt, "ent_e and ent_a (one byte per entry each) fit in slot_c behind the active components");
-__host__ __device__ inline size_t tl_lsov_bytes(int ld) {           // stageO | we | tmask | pref_t, overlaid by ent_val
-    const size_t W = (size_t)sp_ldp(ld) / 32;
-    const size_t span = 16 * (size_t)kTlOwn16 + 8 * 32 + 4 * kTlMaxNodes * W + 2 * kTlMaxNodes * W;
-    const size_t ev = 8 * (size_t)kTlEnt;
-    return ((span > ev ? span : ev) + 15) & ~(size_t)15;
-}
+static_assert(kTlOffSlotC % 8 == 0 && kTlOffAmap % 2 == 0 && kTlOffESoff % 2 == 0, "alignment of the warp region");
+static_assert(kTlAct >= 32, "we (32 doubles) fits where fa goes");
 
 // per-warp shared memory of the tile path (W = ldp / 32 mask words per node)
 __host__ __device__ inline size_t tl_warp_bytes(int ld) {
-    size_t b = 16 * (size_t)kTlStage16;                 // stageN (later xs)
-    b += 16 * (size_t)kTlSlots;                         // fg (later fa | asfm | plist | lcnt | loff)
-    b += tl_lsov_bytes(ld);                             // stageO | we | tmask | pref_t (later ent_val)
-    b += 8 * 8 + 8 * 8;                                 // n_llh, n_G2
-    b += 4 * kTlMaxNodes;                               // n_u
-    b += 2 * 2 * (size_t)kTlSlots;                      // slot_c (later ac | ent_e | ent_a), amap
-    b += 2 * (40 + 40 + 12 + 12 + 12 + 8 + 8);          // e_soff, e_cnt, n_es, n_sb, n_ab, n_m, n_tot
-    b += 2 * 32;                                        // e_io2
-    b += 8 + 8;                                         // n_js, n_want
-    b += (size_t)kTlErow + 2 * 34 + 32;                 // erow, epos, e_ni
-    b += 2 * 8 + 8;                                     // n_sv, n_sl (line search by bounds)
-    return (b + 15) & ~(size_t)15;
+    const size_t W = (size_t)sp_ldp(ld) / 32;
+    const size_t masks = (4 + 2) * kTlMaxNodes * W;     // tmask, pref_t
+    size_t tail = 8 * (size_t)kTlAct;                   // fa
+    if (tail < masks) tail = masks;
+    return (kTlOffFa + tail + 15) & ~(size_t)15;
 }
 __host__ __device__ inline size_t tl_region_bytes(int ld) {
     const size_t t = tl_warp_bytes(ld), g = (sp_gen_warp_bytes(ld) + 15) & ~(size_t)15;
     return t > g ? t : g;
 }
-// block: steps[kMaxSteps] | sumF[ldp] | mbar[kTlMbars] | lns[16 floats] | wpb x warp region
+// block: steps[kMaxSteps] | sumF[ldp] | mbar[kTlMbars] | lns[16 floats] | S2 (+ 8 bytes padding) | wpb x warp region
 __host__ __device__ inline size_t tl_block_smem_bytes(int ld, int wpb) {
-    return sizeof(double) * (kMaxSteps + (size_t)sp_ldp(ld) + kTlMbars + 8) + (size_t)wpb * tl_region_bytes(ld);
+    return sizeof(double) * (kMaxSteps + (size_t)sp_ldp(ld) + kTlMbars + 10) + (size_t)wpb * tl_region_bytes(ld);
 }
 // warps per block: as many resident warps per SM as the shared memory (227 KB, 1 KB reserved per block) allows, in
 // at most kTlMaxBlocks blocks (wide rows run more blocks of fewer warps)
@@ -183,69 +191,73 @@ struct TlWarp {
     const double *s_steps;
     const double *s_sumF;
     const float *s_lns;              // upper bounds of ln(step size) (line search by bounds)
-    double S2_all;                   // sum_c sumF_c^2 (fixed order)
+    const double *s_S2;              // sum_c sumF_c^2 (fixed order)
     EdgeConst ec;
     unsigned char *stageN, *stageO;
-    double2 *fg;
-    double *xs, *ent_val, *we, *n_llh, *n_G2;
+    double *gd, *fa, *stO;
+    double *xs, *ent_val, *asfm, *we, *n_llh, *n_G2;
     unsigned short *n_sv;
     unsigned char *n_sl;
-    int last_ns, last_nw;            // nodes of the last tile that were line-searched / that wanted a line search
+    unsigned char *n_cnt;            // nodes of the last tile that were line-searched / that wanted a line search
     unsigned long long *mbar;
     unsigned int *tmask, *lcnt;
     int *n_u;
-    unsigned short *slot_c, *amap, *loff, *plist, *pref_t, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_tot;
-    unsigned char *ent_e, *ent_a, *erow, *e_ni, *n_want;
+    unsigned short *slot_c, *loff, *plist, *pref_t, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_q;
+    unsigned char *slot_o, *amap, *ent_e, *ent_a, *erow, *e_ni, *n_want;
     unsigned short *epos;
     signed char *n_js;
     int lane, ld, W;
     unsigned parity;
 
+    // the warp region: see the table at kTlOffG
     __device__ __forceinline__ void carve(unsigned char *p, int ld_, int lane_) {
         ld = ld_;
         lane = lane_;
         W = sp_ldp(ld_) / 32;
         parity = 0;
-        stageN = p;                                       p += 16 * (size_t)kTlStage16;
-        xs = reinterpret_cast<double *>(stageN);          // (after the rows have been turned into per-component lists)
-        fg = reinterpret_cast<double2 *>(p);
-        plist = reinterpret_cast<unsigned short *>(p + 24 * (size_t)kTlAct);   // (behind fa | asfm, after the compaction of the active components)
-        lcnt = reinterpret_cast<unsigned int *>(p + kTlLcntOff);                // (phase I, behind the pair list)
-        loff = reinterpret_cast<unsigned short *>(p + kTlLcntOff + 4 * (size_t)kTlAct);
-        p += 16 * (size_t)kTlSlots;
-        {
-            unsigned char *q = p;                         // phases A-H2 ...
-            stageO = q;                                   q += 16 * (size_t)kTlOwn16;
-            we = reinterpret_cast<double *>(q);           q += 8 * 32;
-            tmask = reinterpret_cast<unsigned int *>(q);  q += 4 * (size_t)kTlMaxNodes * W;
-            pref_t = reinterpret_cast<unsigned short *>(q);
-            ent_val = reinterpret_cast<double *>(p);      // ... and phases I-K
-            p += tl_lsov_bytes(ld_);
-        }
-        n_llh = reinterpret_cast<double *>(p);            p += 8 * 8;
-        n_G2 = reinterpret_cast<double *>(p);             p += 8 * 8;
-        n_u = reinterpret_cast<int *>(p);                 p += 4 * kTlMaxNodes;
-        slot_c = reinterpret_cast<unsigned short *>(p);   p += 2 * (size_t)kTlSlots;
-        ent_e = reinterpret_cast<unsigned char *>(slot_c + kTlAct);       // (phases I-K: slot_c is read below A only by then)
+        stageN = p;
+        xs = reinterpret_cast<double *>(p);
+        gd = reinterpret_cast<double *>(p + kTlOffG);
+        ent_val = gd + kTlAct;
+        stageO = p + kTlOffOwn;
+        stO = reinterpret_cast<double *>(stageO);
+        lcnt = reinterpret_cast<unsigned int *>(stageO);
+        loff = reinterpret_cast<unsigned short *>(stageO + 4 * kTlAct);
+        asfm = stO;
+        n_llh = reinterpret_cast<double *>(p + kTlOffLlh);
+        n_G2 = n_llh + 8;
+        slot_c = reinterpret_cast<unsigned short *>(p + kTlOffSlotC);
+        ent_e = reinterpret_cast<unsigned char *>(slot_c + kTlAct);
         ent_a = ent_e + kTlEnt;
-        amap = reinterpret_cast<unsigned short *>(p);     p += 2 * (size_t)kTlSlots;
-        e_soff = reinterpret_cast<unsigned short *>(p);   p += 2 * 40;
-        e_cnt = reinterpret_cast<unsigned short *>(p);    p += 2 * 40;
-        e_io2 = reinterpret_cast<unsigned short *>(p);    p += 2 * 32;     // flat entry t of row e: its index is stageN (as uint16) [(e_io2[e] + t) mod 2^16]
-        n_es = reinterpret_cast<unsigned short *>(p);     p += 2 * 12;
-        n_sb = reinterpret_cast<unsigned short *>(p);     p += 2 * 12;
-        n_ab = reinterpret_cast<unsigned short *>(p);     p += 2 * 12;
-        n_m = reinterpret_cast<unsigned short *>(p);      p += 2 * 8;
-        n_tot = reinterpret_cast<unsigned short *>(p);    p += 2 * 8;
-        epos = reinterpret_cast<unsigned short *>(p);     p += 2 * 34;
-        erow = p;                                         p += (size_t)kTlErow;
-        e_ni = p;                                         p += 32;
-        n_js = reinterpret_cast<signed char *>(p);        p += 8;
-        n_want = p;                                       p += 8;
-        n_sl = p;                                         p += 8;
-        n_sv = reinterpret_cast<unsigned short *>(p);
-        last_ns = 0;
-        last_nw = 0;
+        slot_o = p + kTlOffAmap;
+        amap = slot_o;
+        plist = reinterpret_cast<unsigned short *>(p + kTlOffAmap);
+        erow = p + kTlOffErow;
+        e_soff = reinterpret_cast<unsigned short *>(p + kTlOffESoff);
+        e_cnt = e_soff + 40;
+        e_io2 = reinterpret_cast<unsigned short *>(p + kTlOffEIo2);   // flat entry t of row e: its index is stageN (as uint16) [(e_io2[e] + t) mod 2^16]
+        epos = reinterpret_cast<unsigned short *>(p + kTlOffEpos);
+        e_ni = p + kTlOffENi;
+        n_u = reinterpret_cast<int *>(p + kTlOffNu);
+        n_es = reinterpret_cast<unsigned short *>(p + kTlOffNes);
+        n_sb = n_es + 12;
+        n_ab = n_sb + 12;
+        n_m = n_ab + 12;
+        n_q = n_m + 8;
+        n_sv = n_q + 16;
+        n_js = reinterpret_cast<signed char *>(p + kTlOffNjs);
+        n_want = p + kTlOffNjs + 8;
+        n_sl = p + kTlOffNjs + 16;
+        n_cnt = p + kTlOffNjs + 24;
+        fa = reinterpret_cast<double *>(p + kTlOffFa);
+        we = fa;
+        tmask = reinterpret_cast<unsigned int *>(p + kTlOffFa);
+        pref_t = reinterpret_cast<unsigned short *>(tmask + kTlMaxNodes * W);
+    }
+    // fu of slot `slot`: its own-row value, 0 where the node's row has no entry (phases C2-H)
+    __device__ __forceinline__ double fu_at(int slot) const {
+        const unsigned o = slot_o[slot];
+        return o != 0xffu ? stO[o] : 0.0;
     }
 
     // inclusive scan over the lanes of a group of gs lanes (sub = lane within the group)
@@ -363,7 +375,8 @@ struct TlWarp {
         const int gsh = g << lgs;
         const int gW = g * W;
         const int cu_g = gv ? (int)e_cnt[32 + g] : 0;
-        double *ov = reinterpret_cast<double *>(stageO + 16 * (size_t)(gv ? e_soff[32 + g] : 0));
+        const int ov0 = gv ? 2 * (int)e_soff[32 + g] : 0;                  // the node's own row: stO[ov0 ..]
+        double *ov = stO + ov0;
         unsigned short *oi = sp_idx(ov, (uint32_t)cu_g);
         double fusf = 0.0, fufu = 0.0;
 #pragma unroll 1
@@ -417,18 +430,19 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             total_slots += t;
         }
         if (total_slots > kTlSlots) return false;
-        if (gv && sub == 0) { n_sb[g] = (unsigned short)base_g; n_tot[g] = (unsigned short)tot_g; }
+        if (gv && sub == 0) n_sb[g] = (unsigned short)base_g;
 #pragma unroll 1
-        for (int i = lane; i < total_slots; i += 32) fg[i] = make_double2(0.0, 0.0);
+        for (int i = lane; i < total_slots; i += 32) { gd[i] = 0.0; slot_o[i] = 0xffu; }
         __syncwarp();
         // ---------------- C2. every entry learns its slot (kept in place of the component index) ----------------
+        // (an own entry: its slot learns where the value is, fu_at)
 #pragma unroll 1
         for (int i = sub; i < cu_g; i += gs) {
             const int c = oi[i];
             const int w = c >> 5;
             const unsigned bit = 1u << (c & 31);
             const int slot = base_g + pref_t[gW + w] + __popc(tmask[gW + w] & (bit - 1u));
-            fg[slot].x = ov[i];
+            slot_o[slot] = (unsigned char)(ov0 + i);
             slot_c[slot] = (unsigned short)c;
         }
 BIGCLAM_UNROLL(BIGCLAM_TL_UF)
@@ -448,7 +462,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         double x = 0.0;
         if (lane < ne) {
 #pragma unroll 1
-            for (int i = 0; i < ce; ++i) x = fma(rv[i], fg[ri[i]].x, x);
+            for (int i = 0; i < ce; ++i) x = fma(rv[i], fu_at(ri[i]), x);
         }
         // ---------------- D. edge terms (:166-167), llh_u (:168) ----------------
         double wgt;
@@ -502,7 +516,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
 #pragma unroll 1
                 for (int i = sub; i < cn; i += gs) {
                     const int slot = vi[i];
-                    fg[slot].y = fma(wv, vv[i], fg[slot].y);
+                    gd[slot] = fma(wv, vv[i], gd[slot]);
                 }
             }
             __syncwarp();
@@ -525,10 +539,10 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 bool act = false;
                 if (k < tot_g) {
                     const int slot = base_g + k;
-                    const double2 v = fg[slot];
+                    const double2 v = make_double2(fu_at(slot), gd[slot]);
                     const double sf = s_sumF[slot_c[slot]];
                     const double gr = (v.y - sf) + v.x;
-                    fg[slot].y = gr;
+                    gd[slot] = gr;
                     G2 = fma(gr, gr, G2);
                     SF2 = fma(sf, sf, SF2);
                     act = (v.x > 0.0 || gr > 0.0);
@@ -561,8 +575,8 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 const float g2f = __double2float_ru(G2);
                 r4 = fmaf(2.0f, g2f, sqrtf(g2f) * sqrtf(fmaf(2.0f, __double2float_ru(SF2), 18.0f * __double2float_ru(fufu))) * 1.0001f);
             }
-            // an untouched component has fu = 0 and gradient -sumF_c: its square is part of S2_all
-            G2node = (S2_all - SF2) + G2;
+            // an untouched component has fu = 0 and gradient -sumF_c: its square is part of S2 (*s_S2)
+            G2node = (*s_S2 - SF2) + G2;
             if (gv && sub == 0) n_G2[g] = G2node;
         }
         if (!gv) m_g = 0;
@@ -583,13 +597,15 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         if (prune_on && (e_low || vnear > 0.0f) && lane < ne) {
 #pragma unroll 1
             for (int i = 0; i < ce; ++i) {
-                const double2 v = fg[ri[i]];
+                const int slot = ri[i];
+                const double2 v = make_double2(fu_at(slot), gd[slot]);
                 const double val = rv[i];
                 Dp = fma(val, v.y > 0.0 ? v.y : 0.0, Dp);
                 En = fma(val, (v.y < 0.0 && v.x > 0.0) ? v.y : 0.0, En);
             }
         }
-        // the active components move to the front, in slot order: fg[a] = (fu_c, grad_c), slot_c[a] = c; amap: slot -> a
+        // the active components move to the front, in slot order: fa[a] = fu_c, gd[a] = grad_c, slot_c[a] = c;
+        // amap (on slot_o): slot -> a
         int A = 0;
 #pragma unroll 1
         for (int p0 = 0; p0 < total_slots; p0 += 32) {
@@ -597,23 +613,20 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             const bool ok = p < total_slots;
             double2 v = make_double2(0.0, 0.0);
             int c = 0;
-            if (ok) { v = fg[p]; c = slot_c[p]; }
+            if (ok) { v = make_double2(fu_at(p), gd[p]); c = slot_c[p]; }
             const bool act = ok && (v.x > 0.0 || v.y > 0.0);
             const unsigned bal = __ballot_sync(0xffffffffu, act);
             __syncwarp();                        // every lane has read its slot; the writes land at or below them
             const int an = A + __popc(bal & lt_mask);
-            if (act && an < kTlSlots) { fg[an] = v; slot_c[an] = (unsigned short)c; }
-            if (ok) amap[p] = act ? (unsigned short)an : (unsigned short)0xffffu;
+            if (act && an < kTlAct) { fa[an] = v.x; gd[an] = v.y; slot_c[an] = (unsigned short)c; }
+            if (ok) amap[p] = act ? (unsigned char)an : (unsigned char)0xffu;   // (an > 254 only in a tile that falls back below)
             A += __popc(bal);
             __syncwarp();
         }
         if (A > kTlAct - 1) return false;                      // (one spare: the padding component below)
-        double *asfm = reinterpret_cast<double *>(fg + kTlAct);            // sumF_c - fu_c of the active components
-#pragma unroll 1
-        for (int t = lane; t < A; t += 32) asfm[t] = s_sumF[slot_c[t]] - fg[t].x;
         // padding component A: fu = grad = 0, so every candidate is 0 there and adds exactly nothing — the lockstep loops
         // of the line search read it instead of predicating their bodies
-        if (lane == 0) { fg[A] = make_double2(0.0, 0.0); asfm[A] = 0.0; }
+        if (lane == 0) { fa[A] = 0.0; gd[A] = 0.0; }
         __syncwarp();
         // ---------------- H2. bounds: which (node, candidate) pairs can pass the Armijo test at all ----------------
         // Most candidates can be PROVEN to fail (:181) from what the PRE block already has.  Write the node's objective
@@ -640,7 +653,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         // the results are the same bits as those of the exhaustive search (BIGCLAM_F_LS_EXHAUSTIVE, tests/test_gpu_prune.py).
         // Mapping: lane = edge for the per-edge terms, then the lanes of a node's group share its candidates.
         const bool prune = prune_on;
-        float2 *we2 = reinterpret_cast<float2 *>(we);          // (the weights w_e are not needed any more)
+        float2 *we2 = reinterpret_cast<float2 *>(stO);         // (the own rows are not needed any more)
         if (prune) {
             float lnthr = 3.0e38f, Lp = 0.0f;                  // H_e(s) = 0 up to ln s = lnthr, <= min(cap, ln s + Lp) beyond
             if (vnear > 0.0f) {
@@ -751,8 +764,8 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         // the nodes that are line-searched at all, in tile order
         const unsigned svmask = __ballot_sync(0xffffffffu, lane < nn && n_sv[lane < nn ? lane : 0] != 0);
         const int ns = __popc(svmask);
-        last_ns = ns;
-        last_nw = __popc(__ballot_sync(0xffffffffu, lane < nn && n_want[lane < nn ? lane : 0] != 0));
+        const int nw = __popc(__ballot_sync(0xffffffffu, lane < nn && n_want[lane < nn ? lane : 0] != 0));
+        if (lane == 0) { n_cnt[0] = (unsigned char)ns; n_cnt[1] = (unsigned char)nw; }
         if (lane < nn) {
             n_js[lane] = -1;
             if ((svmask >> lane) & 1u) n_sl[__popc(svmask & lt_mask)] = (unsigned char)lane;
@@ -781,7 +794,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
 BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 for (int t = (int)epos[n_es[na]] + lane; t < thi; t += 32) {
                     const unsigned an = amap[stN16[(unsigned short)(e_io2[erow[t]] + t)]];
-                    if (an != 0xffffu) atomicAdd(lcnt + an, 1u);
+                    if (an != 0xffu) atomicAdd(lcnt + an, 1u);
                 }
             }
             __syncwarp();
@@ -814,6 +827,10 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 ent_a[TE] = (unsigned char)A;
             }
             __syncwarp();
+            if (lane < nn && ((svmask >> lane) & 1u)) {            // the node's range of entries (loff dies with phase I)
+                n_q[2 * lane] = loff[n_ab[lane]];
+                n_q[2 * lane + 1] = loff[n_ab[lane] + n_m[lane]];
+            }
             rem = svmask;
 #pragma unroll 1
             while (rem) {
@@ -826,7 +843,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                     const double *vv = reinterpret_cast<const double *>(stageN + 16 * (size_t)e_soff[row]);
                     const int i = t - (int)epos[row];
                     const unsigned an = amap[stN16[(unsigned short)(e_io2[row] + t)]];
-                    if (an != 0xffffu) {
+                    if (an != 0xffu) {
                         const unsigned q = atomicAdd(lcnt + an, 1u);
                         ent_val[q] = vv[i];
                         ent_e[q] = (unsigned char)row;
@@ -835,6 +852,9 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 }
             }
             __syncwarp();
+            // sumF_c - fu_c of the active components (on lcnt | loff), the padding component A included
+#pragma unroll 1
+            for (int t = lane; t <= A; t += 32) asfm[t] = (t < A) ? s_sumF[slot_c[t]] - fa[t] : 0.0;
             // ---------------- J. line search (:172-180), two line-searched nodes at a time: lane = (node, trial j) ----------------
             // One loop over the node's active components gives, per candidate: newfu.sfT and newfu.newfu (:176,:180) and,
             // through the components' entry lists, newfu.fv of every edge (xs[edge][trial], component order ascending).
@@ -849,7 +869,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 const bool mine = nv && (((unsigned)n_sv[node] >> j) & 1u);     // (a pair that cannot pass is not evaluated)
                 const int e0 = nv ? (int)n_es[node] : 0, dn = nv ? (int)n_es[node + 1] - e0 : 0;
                 const int t0 = nv ? (int)n_ab[node] : 0, mm = nv ? (int)n_m[node] : 0;
-                const int q0 = nv ? (int)loff[t0] : 0, nq = nv ? (int)loff[t0 + mm] - q0 : 0;
+                const int q0 = nv ? (int)n_q[2 * node] : 0, nq = nv ? (int)n_q[2 * node + 1] - q0 : 0;
 #pragma unroll 1
                 for (int r = 0; r < dn; ++r) xs[(e0 + r) * 16 + j] = 0.0;       // (each cell belongs to one lane)
                 // the two half-warps (two nodes) walk in lockstep: common trip counts, padded with a component / an entry that add nothing
@@ -860,7 +880,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
 BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                 for (int t = 0; t < mmax; ++t) {
                     const int ti = (t < mm) ? t0 + t : A;                   // (A: the padding component, adds +0.0)
-                    const double2 v = fg[ti];
+                    const double2 v = make_double2(fa[ti], gd[ti]);
                     const double nf = need_hi ? clamp_step0(v.x, s, v.y, max_f) : clamp_step0_lo(v.x, s, v.y);
                     const double sf = asfm[ti] + nf;                        // sfT = (sumF - fu) + newfu   (:176)
                     a1 = fma(nf, sf, a1);
@@ -869,7 +889,8 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
 BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                 for (int k = 0; k < qmax; ++k) {
                     const int qq = (k < nq) ? q0 + k : TE;                  // (TE: the padding entry, scratch cell, value 0)
-                    const double2 v = fg[ent_a[qq]];
+                    const int ea = ent_a[qq];
+                    const double2 v = make_double2(fa[ea], gd[ea]);
                     const double nf = need_hi ? clamp_step0(v.x, s, v.y, max_f) : clamp_step0_lo(v.x, s, v.y);
                     double *cell = xs + (int)ent_e[qq] * 16 + j;
                     *cell = fma(nf, ent_val[qq], *cell);
@@ -940,7 +961,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
             const int t = t0 + sub;
             bool isnz = false, ch = false;
             if (js >= 0 && t < m_g) {
-                const double2 v = fg[ab_g + t];
+                const double2 v = make_double2(fa[ab_g + t], gd[ab_g + t]);
                 const double nr = clamp_step(v.x, sstar, v.y, a->min_f, max_f);
                 isnz = nr != 0.0;
                 ch = v.x != nr;
@@ -981,7 +1002,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                 double nr = 0.0, f = 0.0;
                 int c = 0;
                 if (js >= 0 && t < m_g) {
-                    const double2 v = fg[ab_g + t];
+                    const double2 v = make_double2(fa[ab_g + t], gd[ab_g + t]);
                     c = slot_c[ab_g + t];
                     f = v.x;
                     nr = clamp_step(f, sstar, v.y, a->min_f, max_f);
@@ -1111,7 +1132,8 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     double *s_sumF = s_steps + kMaxSteps;
     unsigned long long *s_mbar = reinterpret_cast<unsigned long long *>(s_sumF + ldp);
     float *s_lns = reinterpret_cast<float *>(s_mbar + kTlMbars);          // 16 floats
-    unsigned char *wbase = reinterpret_cast<unsigned char *>(s_mbar + kTlMbars + 8) + (size_t)wib * tl_region_bytes(ld);
+    double *s_S2 = reinterpret_cast<double *>(s_mbar + kTlMbars + 8);
+    unsigned char *wbase = reinterpret_cast<unsigned char *>(s_mbar + kTlMbars + 10) + (size_t)wib * tl_region_bytes(ld);
 
 #pragma unroll 1
     for (int i = threadIdx.x; i < ldp; i += nthreads) s_sumF[i] = (i < ld) ? a.sumF[i] : 0.0;
@@ -1122,11 +1144,17 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
         const float t = (sfu > 0.0f) ? __log2f(sfu) : -3.0e38f;
         s_lns[threadIdx.x] = (sfu > 0.0f) ? t * 0.69314718f + fmaf(1.0e-6f, fabsf(t), 1.0e-4f) : -3.0e38f;
     }
+    if (wib == 0) {
+        // S2 = sum_c sumF_c^2 in a fixed order, once per block (read in phase H, not held in a register)
+        double S2 = 0.0;
+        for (int c = lane; c < ldp; c += 32) {
+            const double v = (c < ld) ? a.sumF[c] : 0.0;
+            S2 = fma(v, v, S2);
+        }
+        S2 = warp_sum(S2);
+        if (lane == 0) *s_S2 = S2;
+    }
     __syncthreads();
-    // S2_all = sum_c sumF_c^2 in a fixed order (every warp computes the same bits)
-    double S2 = 0.0;
-    for (int c = lane; c < ldp; c += 32) S2 = fma(s_sumF[c], s_sumF[c], S2);
-    S2 = warp_sum(S2);
 
     SpGen<false> G;
     G.a = &a;
@@ -1142,7 +1170,7 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     T.s_steps = s_steps;
     T.s_sumF = s_sumF;
     T.s_lns = s_lns;
-    T.S2_all = S2;
+    T.s_S2 = s_S2;
     T.ec = G.ec;
     T.carve(wbase, ld, lane);
     T.mbar = s_mbar + wib;
@@ -1161,11 +1189,12 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
         }
     }
 
-    const unsigned int n_items = (unsigned int)sp.n_gen + (unsigned int)sp.ntiles;
+    // items: n_gen general-path nodes, then ntiles tiles (the bounds are compared one by one, straight from the
+    // launch arguments: their sum would hold a register across the whole loop)
     unsigned int item = 0;
     if (lane == 0) item = atomicAdd(a.work_counter, 1u);
     item = __shfl_sync(0xffffffffu, item, 0);
-    while (item < n_items) {
+    while (item < (unsigned int)sp.n_gen || item - (unsigned int)sp.n_gen < (unsigned int)sp.ntiles) {
         unsigned int nxt = 0;
         if (lane == 0) nxt = atomicAdd(a.work_counter, 1u);
         // nodes for the general path: the item itself, or the nodes of a tile that did not fit (one call site)
@@ -1178,7 +1207,7 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
             const bool done = T.template run<kPush>(tm);
             if (sp.stats != nullptr && lane == 0) {
                 atomicAdd(sp.stats + (done ? 0 : 1), 1u);
-                if (done && a.do_linesearch) { atomicAdd(sp.stats + 2, (unsigned)T.last_ns); atomicAdd(sp.stats + 3, (unsigned)T.last_nw); }
+                if (done && a.do_linesearch) { atomicAdd(sp.stats + 2, (unsigned)T.n_cnt[0]); atomicAdd(sp.stats + 3, (unsigned)T.n_cnt[1]); }
             }
             gen_cnt = done ? 0 : tm.nn;
             gen_pos = tm.pos0;
