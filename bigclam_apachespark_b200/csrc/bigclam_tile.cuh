@@ -59,10 +59,11 @@ constexpr int kTlMaxEdges = 32;
 #endif
 #define BIGCLAM_PRAGMA(x) _Pragma(#x)
 #define BIGCLAM_UNROLL(n) BIGCLAM_PRAGMA(unroll n)
-// one block of 18 warps per SM at K <= 256: buffers whose lifetimes do not overlap share bytes (12.2 KB per warp up to
-// K = 832, see the warp region below), and the block's steps and sumF are held once per SM
+// one block of 20 warps per SM (five on each of the four sub-partitions) at K <= 320: buffers whose lifetimes do not
+// overlap share bytes (11.2 KB per warp at every K of the tile path, see the warp region below), and the block's steps
+// and sumF are held once per SM
 #ifndef BIGCLAM_TL_WARPS
-#define BIGCLAM_TL_WARPS 18
+#define BIGCLAM_TL_WARPS 20
 #endif
 #ifndef BIGCLAM_TL_BLOCKS
 #define BIGCLAM_TL_BLOCKS 1
@@ -85,13 +86,14 @@ static_assert(2 * kTlOwn16 < 255, "own-entry indices of the slots are bytes (0xf
 
 // The warp region of the tile path.  Buffers whose lifetimes do not overlap share bytes (phases: TlWarp::run):
 //   stageN   neighbour rows  A-I                  | xs (edge x trial)  J-K
-//   gd       g per slot  E-H                      | g of the active components [kTlAct]  H-L, ent_val behind them  I-J
-//   stageO   own rows  A-H (fu of a slot is read through slot_o)  | we2  H2 | lcnt, loff  I | asfm  J
+//   gd       tmask | pref_t (48 B per mask word of a node)  A-C2 | g per slot  G-H
+//            | g of the active components [kTlAct]  H-L; behind them we2  H2, fu on its way to fa  I, ent_val  I-J
+//   stageO   own rows  A-I (fu through slot_o, then through fo)   | fa (fu of the active components [kTlAct])  I-L
 //   slot_c   component of a slot  C2-L (below A only after H)     | ent_e, ent_a behind kTlAct  I-J
 //   slot_o   own-entry index of a slot (byte)  C2-H               | amap (slot -> active index, byte)  H-I   | plist  J
 //   erow, e_soff, e_cnt, e_io2 (entry -> row, rows' places)  A-I                                          | plist  J
-//   fa       fu of the active components [kTlAct]  H-L;  before: tmask | pref_t  A-C2, we  D-G
-// Everything but the tail (fa, or tmask | pref_t: 48 B per mask word of a node) is at a fixed offset.
+//   tail     we  D-G | fo (own-entry index of an active component, byte)  H-I | lcnt (byte)  I
+// (sumF - fu of an active component is computed where phase J reads it.)
 constexpr int kTlOffG = 16 * kTlStage16;
 constexpr int kTlOffOwn = kTlOffG + 8 * kTlSlots;
 constexpr int kTlOffLlh = kTlOffOwn + 16 * kTlOwn16;                  // n_llh, n_G2 [8 doubles each]
@@ -105,26 +107,25 @@ constexpr int kTlOffENi = kTlOffEpos + 2 * 34;
 constexpr int kTlOffNu = (kTlOffENi + 32 + 3) & ~3;                   // n_u [8 int]
 constexpr int kTlOffNes = kTlOffNu + 4 * kTlMaxNodes;                 // n_es, n_sb, n_ab [12 u16 each], n_m [8], n_q [16], n_sv [8]
 constexpr int kTlOffNjs = kTlOffNes + 2 * (12 + 12 + 12 + 8 + 16 + 8); // n_js, n_want, n_sl [8 bytes each], n_cnt [2]
-constexpr int kTlOffFa = (kTlOffNjs + 3 * 8 + 2 + 7) & ~7;
+constexpr int kTlOffTail = (kTlOffNjs + 3 * 8 + 2 + 7) & ~7;
+constexpr int kTlTail = 8 * kTlMaxEdges;                              // we: one double per edge
 static_assert(8 * kTlAct + 8 * kTlEnt <= 8 * kTlSlots, "ent_val fits in gd behind the gradients of the active components");
-static_assert(16 * kTlOwn16 >= 4 * kTlAct + 2 * (kTlAct + 2) && 16 * kTlOwn16 >= 8 * kTlAct && 16 * kTlOwn16 >= 8 * 32,
-              "stageO holds lcnt | loff, then asfm, and we2");
+static_assert((4 + 2) * kTlMaxNodes * (kSpWideLd / 32) <= 8 * kTlSlots, "tmask | pref_t fit in gd at every K of the tile path");
+static_assert(16 * kTlOwn16 >= 8 * kTlAct, "fa fits on stageO");
+static_assert(kTlTail >= kTlAct, "fo and lcnt (one byte per active component) fit where we goes");
+static_assert(8 * (kTlSlots - kTlAct) >= 8 * kTlMaxEdges && 8 * (kTlSlots - kTlAct) >= 8 * kTlAct,
+              "we2 (a float2 per edge) and fu on its way to fa fit in gd behind the gradients of the active components");
+static_assert(kTlMaxEdges < 256 && kTlEnt <= 256,
+              "lcnt: byte counters (a list has at most one entry per edge of its node) and byte cursors (below TE < kTlEnt)");
 static_assert(kTlOffEIo2 + 2 * 32 - kTlOffAmap >= 2 * 16 * kTlMaxEdges, "the pair list of a line-search round fits on amap .. e_io2");
 static_assert(kTlSlots - kTlAct >= kTlEnt, "ent_e and ent_a (one byte per entry each) fit in slot_c behind the active components");
-static_assert(kTlOffSlotC % 8 == 0 && kTlOffAmap % 2 == 0 && kTlOffESoff % 2 == 0, "alignment of the warp region");
-static_assert(kTlAct >= 32, "we (32 doubles) fits where fa goes");
+static_assert(kTlOffSlotC % 8 == 0 && kTlOffAmap % 2 == 0 && kTlOffESoff % 2 == 0 && kTlOffTail % 8 == 0, "alignment of the warp region");
 
-// per-warp shared memory of the tile path (W = ldp / 32 mask words per node)
-__host__ __device__ inline size_t tl_warp_bytes(int ld) {
-    const size_t W = (size_t)sp_ldp(ld) / 32;
-    const size_t masks = (4 + 2) * kTlMaxNodes * W;     // tmask, pref_t
-    size_t tail = 8 * (size_t)kTlAct;                   // fa
-    if (tail < masks) tail = masks;
-    return (kTlOffFa + tail + 15) & ~(size_t)15;
-}
+// per-warp shared memory of the tile path (the same at every K of it: the K-sized masks live in gd)
+constexpr size_t kTlWarpBytes = (kTlOffTail + kTlTail + 15) & ~(size_t)15;
 __host__ __device__ inline size_t tl_region_bytes(int ld) {
-    const size_t t = tl_warp_bytes(ld), g = (sp_gen_warp_bytes(ld) + 15) & ~(size_t)15;
-    return t > g ? t : g;
+    const size_t g = (sp_gen_warp_bytes(ld) + 15) & ~(size_t)15;
+    return kTlWarpBytes > g ? kTlWarpBytes : g;
 }
 // block: steps[kMaxSteps] | sumF[ldp] | mbar[kTlMbars] | lns[16 floats] | S2 (+ 8 bytes padding) | wpb x warp region
 __host__ __device__ inline size_t tl_block_smem_bytes(int ld, int wpb) {
@@ -195,15 +196,15 @@ struct TlWarp {
     EdgeConst ec;
     unsigned char *stageN, *stageO;
     double *gd, *fa, *stO;
-    double *xs, *ent_val, *asfm, *we, *n_llh, *n_G2;
+    double *xs, *ent_val, *we, *n_llh, *n_G2;
     unsigned short *n_sv;
     unsigned char *n_sl;
     unsigned char *n_cnt;            // nodes of the last tile that were line-searched / that wanted a line search
     unsigned long long *mbar;
-    unsigned int *tmask, *lcnt;
+    unsigned int *tmask;
     int *n_u;
-    unsigned short *slot_c, *loff, *plist, *pref_t, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_q;
-    unsigned char *slot_o, *amap, *ent_e, *ent_a, *erow, *e_ni, *n_want;
+    unsigned short *slot_c, *plist, *pref_t, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_q;
+    unsigned char *slot_o, *amap, *fo, *lcnt, *ent_e, *ent_a, *erow, *e_ni, *n_want;
     unsigned short *epos;
     signed char *n_js;
     int lane, ld, W;
@@ -219,11 +220,11 @@ struct TlWarp {
         xs = reinterpret_cast<double *>(p);
         gd = reinterpret_cast<double *>(p + kTlOffG);
         ent_val = gd + kTlAct;
+        tmask = reinterpret_cast<unsigned int *>(gd);
+        pref_t = reinterpret_cast<unsigned short *>(tmask + kTlMaxNodes * W);
         stageO = p + kTlOffOwn;
         stO = reinterpret_cast<double *>(stageO);
-        lcnt = reinterpret_cast<unsigned int *>(stageO);
-        loff = reinterpret_cast<unsigned short *>(stageO + 4 * kTlAct);
-        asfm = stO;
+        fa = stO;
         n_llh = reinterpret_cast<double *>(p + kTlOffLlh);
         n_G2 = n_llh + 8;
         slot_c = reinterpret_cast<unsigned short *>(p + kTlOffSlotC);
@@ -249,15 +250,17 @@ struct TlWarp {
         n_want = p + kTlOffNjs + 8;
         n_sl = p + kTlOffNjs + 16;
         n_cnt = p + kTlOffNjs + 24;
-        fa = reinterpret_cast<double *>(p + kTlOffFa);
-        we = fa;
-        tmask = reinterpret_cast<unsigned int *>(p + kTlOffFa);
-        pref_t = reinterpret_cast<unsigned short *>(tmask + kTlMaxNodes * W);
+        we = reinterpret_cast<double *>(p + kTlOffTail);
+        fo = p + kTlOffTail;
+        lcnt = p + kTlOffTail;
     }
-    // fu of slot `slot`: its own-row value, 0 where the node's row has no entry (phases C2-H)
-    __device__ __forceinline__ double fu_at(int slot) const {
-        const unsigned o = slot_o[slot];
-        return o != 0xffu ? stO[o] : 0.0;
+    // fu of own-entry index o (slot_o, fo): its own-row value, 0 where the node's row has no entry (phases C2-H)
+    __device__ __forceinline__ double fu_of(unsigned o) const { return o != 0xffu ? stO[o] : 0.0; }
+    __device__ __forceinline__ double fu_at(int slot) const { return fu_of(slot_o[slot]); }
+    // adds 1 to the byte lcnt[i] through the 32-bit word that holds it (no byte carries over: see kTlEnt); returns its old value
+    __device__ __forceinline__ unsigned lcnt_inc(unsigned i) const {
+        const unsigned sh = 8u * (i & 3u);
+        return (atomicAdd(reinterpret_cast<unsigned int *>(lcnt) + (i >> 2), 1u << sh) >> sh) & 0xffu;
     }
 
     // inclusive scan over the lanes of a group of gs lanes (sub = lane within the group)
@@ -432,7 +435,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         if (total_slots > kTlSlots) return false;
         if (gv && sub == 0) n_sb[g] = (unsigned short)base_g;
 #pragma unroll 1
-        for (int i = lane; i < total_slots; i += 32) { gd[i] = 0.0; slot_o[i] = 0xffu; }
+        for (int i = lane; i < total_slots; i += 32) slot_o[i] = 0xffu;
         __syncwarp();
         // ---------------- C2. every entry learns its slot (kept in place of the component index) ----------------
         // (an own entry: its slot learns where the value is, fu_at)
@@ -503,6 +506,8 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             return true;
         }
         if (gv && sub == 0) n_llh[g] = llh_g;
+#pragma unroll 1
+        for (int i = lane; i < total_slots; i += 32) gd[i] = 0.0;      // (gd held tmask | pref_t up to C2)
         __syncwarp();
         // ---------------- G. sum_v fv / (1 - p) (:167-168), edge by edge in CSR order ----------------
 #pragma unroll 1
@@ -604,7 +609,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 En = fma(val, (v.y < 0.0 && v.x > 0.0) ? v.y : 0.0, En);
             }
         }
-        // the active components move to the front, in slot order: fa[a] = fu_c, gd[a] = grad_c, slot_c[a] = c;
+        // the active components move to the front, in slot order: fo[a] = own-entry index, gd[a] = grad_c, slot_c[a] = c;
         // amap (on slot_o): slot -> a
         int A = 0;
 #pragma unroll 1
@@ -618,16 +623,13 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             const unsigned bal = __ballot_sync(0xffffffffu, act);
             __syncwarp();                        // every lane has read its slot; the writes land at or below them
             const int an = A + __popc(bal & lt_mask);
-            if (act && an < kTlAct) { fa[an] = v.x; gd[an] = v.y; slot_c[an] = (unsigned short)c; }
+            // (slot_o[p] is read again rather than held across the barrier: amap[p] replaces it only below)
+            if (act && an < kTlAct) { fo[an] = slot_o[p]; gd[an] = v.y; slot_c[an] = (unsigned short)c; }
             if (ok) amap[p] = act ? (unsigned char)an : (unsigned char)0xffu;   // (an > 254 only in a tile that falls back below)
             A += __popc(bal);
             __syncwarp();
         }
-        if (A > kTlAct - 1) return false;                      // (one spare: the padding component below)
-        // padding component A: fu = grad = 0, so every candidate is 0 there and adds exactly nothing — the lockstep loops
-        // of the line search read it instead of predicating their bodies
-        if (lane == 0) { fa[A] = 0.0; gd[A] = 0.0; }
-        __syncwarp();
+        if (A > kTlAct - 1) return false;                      // (one spare: the padding component, see I)
         // ---------------- H2. bounds: which (node, candidate) pairs can pass the Armijo test at all ----------------
         // Most candidates can be PROVEN to fail (:181) from what the PRE block already has.  Write the node's objective
         // as phi(nf) = sum_v T(nf.fv) - nf.(sumF - fu), T(x) = S(x) + x, S(x) = log(1 - clamp(exp(-x))) (:166,:179): S is
@@ -653,7 +655,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         // the results are the same bits as those of the exhaustive search (BIGCLAM_F_LS_EXHAUSTIVE, tests/test_gpu_prune.py).
         // Mapping: lane = edge for the per-edge terms, then the lanes of a node's group share its candidates.
         const bool prune = prune_on;
-        float2 *we2 = reinterpret_cast<float2 *>(stO);         // (the own rows are not needed any more)
+        float2 *we2 = reinterpret_cast<float2 *>(ent_val);     // (bytes of gd that are free from the compaction to phase I)
         if (prune) {
             float lnthr = 3.0e38f, Lp = 0.0f;                  // H_e(s) = 0 up to ln s = lnthr, <= min(cap, ln s + Lp) beyond
             if (vnear > 0.0f) {
@@ -772,9 +774,21 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         }
         __syncwarp();
         if (ns > 0) {
+            // fa[a] = fu_c onto the own rows' bytes, through ent_val's bytes (free until the fill below).  Padding component A:
+            // fu = grad = 0, so every candidate is 0 there and adds exactly nothing — the lockstep loops of the line search
+            // read it instead of predicating their bodies
+#pragma unroll 1
+            for (int t = lane; t <= A; t += 32) ent_val[t] = (t < A) ? fu_of(fo[t]) : 0.0;
+            if (lane == 0) gd[A] = 0.0;
+            __syncwarp();
+#pragma unroll 1
+            for (int t = lane; t <= A; t += 32) fa[t] = ent_val[t];
+            __syncwarp();
             // ---------------- I. the neighbours' entries on active components, listed per component ----------------
             // (only for the nodes that are line-searched: flat loops over runs of consecutive such nodes — their edges,
-            // entries and active components are contiguous)
+            // entries and active components are contiguous.)  lcnt[a] counts the entries of component a, then holds the
+            // write cursor of its list: one byte each, as a list has at most one entry per edge of its node and the cursors
+            // stay below TE <= kTlEnt - 1.
             unsigned rem = svmask;
 #pragma unroll 1
             while (rem) {
@@ -782,7 +796,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 rem &= ~(((1u << len) - 1u) << na);
                 const int ahi = (int)n_ab[na + len - 1] + (int)n_m[na + len - 1];
 #pragma unroll 1
-                for (int t = (int)n_ab[na] + lane; t < ahi; t += 32) lcnt[t] = 0u;
+                for (int t = (int)n_ab[na] + lane; t < ahi; t += 32) lcnt[t] = 0;
             }
             __syncwarp();
             rem = svmask;
@@ -794,7 +808,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
 BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 for (int t = (int)epos[n_es[na]] + lane; t < thi; t += 32) {
                     const unsigned an = amap[stN16[(unsigned short)(e_io2[erow[t]] + t)]];
-                    if (an != 0xffu) atomicAdd(lcnt + an, 1u);
+                    if (an != 0xffu) lcnt_inc(an);
                 }
             }
             __syncwarp();
@@ -815,10 +829,9 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                         const int v = __shfl_up_sync(0xffffffffu, incl, o);
                         if (lane >= o) incl += v;
                     }
-                    if (t < ahi) { loff[t] = (unsigned short)(TE + incl - c); lcnt[t] = (unsigned int)(TE + incl - c); }
+                    if (t < ahi) lcnt[t] = (unsigned char)(TE + incl - c);
                     TE += __shfl_sync(0xffffffffu, incl, 31);
                 }
-                if (lane == 0) loff[ahi] = (unsigned short)TE;          // end of the run's last list (a following run starts there or later)
             }
             if (TE > kTlEnt - 1) return false;
             if (lane == 0) {
@@ -827,10 +840,10 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 ent_a[TE] = (unsigned char)A;
             }
             __syncwarp();
-            if (lane < nn && ((svmask >> lane) & 1u)) {            // the node's range of entries (loff dies with phase I)
-                n_q[2 * lane] = loff[n_ab[lane]];
-                n_q[2 * lane + 1] = loff[n_ab[lane] + n_m[lane]];
-            }
+            // the node's range of entries: from the start of its first list here, to the end of its last one after the fill
+            const bool q_lane = lane < nn && ((svmask >> lane) & 1u);
+            if (q_lane) n_q[2 * lane] = n_m[lane] > 0 ? lcnt[n_ab[lane]] : 0;
+            __syncwarp();
             rem = svmask;
 #pragma unroll 1
             while (rem) {
@@ -844,7 +857,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                     const int i = t - (int)epos[row];
                     const unsigned an = amap[stN16[(unsigned short)(e_io2[row] + t)]];
                     if (an != 0xffu) {
-                        const unsigned q = atomicAdd(lcnt + an, 1u);
+                        const unsigned q = lcnt_inc(an);
                         ent_val[q] = vv[i];
                         ent_e[q] = (unsigned char)row;
                         ent_a[q] = (unsigned char)an;
@@ -852,9 +865,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 }
             }
             __syncwarp();
-            // sumF_c - fu_c of the active components (on lcnt | loff), the padding component A included
-#pragma unroll 1
-            for (int t = lane; t <= A; t += 32) asfm[t] = (t < A) ? s_sumF[slot_c[t]] - fa[t] : 0.0;
+            if (q_lane) n_q[2 * lane + 1] = n_m[lane] > 0 ? lcnt[n_ab[lane] + n_m[lane] - 1] : 0;
             // ---------------- J. line search (:172-180), two line-searched nodes at a time: lane = (node, trial j) ----------------
             // One loop over the node's active components gives, per candidate: newfu.sfT and newfu.newfu (:176,:180) and,
             // through the components' entry lists, newfu.fv of every edge (xs[edge][trial], component order ascending).
@@ -882,7 +893,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                     const int ti = (t < mm) ? t0 + t : A;                   // (A: the padding component, adds +0.0)
                     const double2 v = make_double2(fa[ti], gd[ti]);
                     const double nf = need_hi ? clamp_step0(v.x, s, v.y, max_f) : clamp_step0_lo(v.x, s, v.y);
-                    const double sf = asfm[ti] + nf;                        // sfT = (sumF - fu) + newfu   (:176)
+                    const double sf = ((t < mm) ? s_sumF[slot_c[ti]] - v.x : 0.0) + nf;   // sfT = (sumF - fu) + newfu   (:176)
                     a1 = fma(nf, sf, a1);
                     b1 = fma(nf, nf, b1);
                 }
