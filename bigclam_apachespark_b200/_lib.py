@@ -137,6 +137,8 @@ SIGNATURES = {
     "bigclam_conductance_seeds": (C.c_int, [_i64, _vp, _vp, _vp, _vp, _pi64]),
     "bigclam_conductance_seeds_gpu": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _vp, _pi64]),
     "bigclam_init_neighbor_com_F": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _i64, _i32, C.c_uint64, _vp]),
+    "bigclam_init_F": (C.c_int, [_vp, _vp, _i64, _i32, C.c_uint64]),
+    "bigclam_multi_init_F": (C.c_int, [_vp, _vp, _i64, _i32, C.c_uint64]),
     "bigclam_device_count": (C.c_int, []),
     "bigclam_version": (C.c_char_p, []),
 }

@@ -896,6 +896,161 @@ extern "C" int bigclam_set_F_csr(bigclam_ctx *ctx, const int64_t *indptr, const 
     return BIGCLAM_OK;
 }
 
+// The padding sequence of initNeighborComF as GF(2) matrices (bigclam_sparse.cuh): 64 columns each, column i = the
+// image of bit i.  tabs = byte tables of T^(2^j) for j < njump (2^njump > n), then of T^n; returns njump.
+static void gf2_mul(const uint64_t *A, const uint64_t *B, uint64_t *out) {
+    for (int i = 0; i < 64; ++i) {
+        uint64_t r = 0;
+        for (int j = 0; j < 64; ++j)
+            if ((B[i] >> j) & 1u) r ^= A[j];
+        out[i] = r;
+    }
+}
+static void gf2_tables(const uint64_t *M, uint64_t *tab) {
+    for (int b = 0; b < 8; ++b) {
+        uint64_t *t = tab + b * 256;
+        t[0] = 0;
+        for (int x = 1; x < 256; ++x) t[x] = t[x & (x - 1)] ^ M[8 * b + __builtin_ctz((unsigned)x)];
+    }
+}
+static int xs_jump_tables(int64_t n, std::vector<uint64_t> &tabs) {
+    int njump = 0;
+    while (((int64_t)1 << njump) <= n) ++njump;
+    tabs.assign((size_t)(njump + 1) * kGf2Tab, 0);
+    uint64_t P[64], N[64], R[64];
+    for (int i = 0; i < 64; ++i) { P[i] = xs_next(1ull << i); N[i] = 1ull << i; }
+    for (int j = 0; j < njump; ++j) {               // P = T^(2^j), N = T^(n mod 2^j)
+        gf2_tables(P, tabs.data() + (size_t)j * kGf2Tab);
+        if ((n >> j) & 1) { gf2_mul(P, N, R); std::copy(R, R + 64, N); }
+        gf2_mul(P, P, R);
+        std::copy(R, R + 64, P);
+    }
+    gf2_tables(N, tabs.data() + (size_t)njump * kGf2Tab);
+    return njump;
+}
+
+// Device scratch of one call, freed on every return path.
+struct DevScratch {
+    std::vector<void *> p;
+    ~DevScratch() { for (void *q : p) cudaFree(q); }
+    template <class T> cudaError_t alloc(T **out, size_t count) {
+        *out = nullptr;
+        cudaError_t e = cudaMalloc(out, sizeof(T) * std::max<size_t>(1, count));
+        if (e == cudaSuccess) p.push_back((void *)*out);
+        return e;
+    }
+};
+
+// out[0 .. n] = the exclusive scan of cnt (words: of sp_words(cnt)); out[n] = the total.
+static int scan_counts(bigclam_ctx *ctx, DevScratch &ds, const unsigned *cnt, int64_t n, int words, uint64_t *out) {
+    const int64_t nchunks = (n + kScanChunk - 1) / kScanChunk;
+    uint64_t *chunk = nullptr;
+    CU(ds.alloc(&chunk, (size_t)nchunks));
+    scan_chunks_kernel<<<(unsigned)nchunks, kScanThreads, 0, ctx->stream>>>(cnt, n, words, chunk);
+    scan_top_kernel<<<1, kScanThreads, 0, ctx->stream>>>(chunk, nchunks, out + n);
+    scan_apply_kernel<<<(unsigned)nchunks, kScanThreads, 0, ctx->stream>>>(cnt, n, words, chunk, out);
+    CU(cudaGetLastError());
+    return BIGCLAM_OK;
+}
+
+// initNeighborComF(K) (bigclam4-7.scala:81-108) built on the device, straight into the context: the state
+// bigclam_init_neighbor_com_F + bigclam_set_F leave, from the context's own graph and without an n x K array.
+extern "C" int bigclam_init_F(bigclam_ctx *ctx, const int32_t *ranked_seeds, int64_t n_ranked, int32_t include_self, uint64_t pad_seed) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    if (n_ranked < 0 || (n_ranked > 0 && ranked_seeds == nullptr))
+        return fail(ctx, BIGCLAM_EINVAL, "bigclam_init_F: ranked_seeds is NULL or n_ranked < 0");
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k, ld = ctx->ld;
+    // S = Sbc.value.take(K) (:83), in id order (:85-86)
+    std::vector<int32_t> S(ranked_seeds, ranked_seeds + std::min<int64_t>(k, n_ranked));
+    std::sort(S.begin(), S.end());
+    uint64_t npairs = 0;
+    for (int32_t s : S) {
+        if (s < 0 || s >= n) return fail(ctx, BIGCLAM_EINVAL, "bigclam_init_F: seed %d outside [0, %lld)", s, (long long)n);
+        npairs += (uint64_t)(ctx->h_rowptr[(size_t)s + 1] - ctx->h_rowptr[(size_t)s]) + (include_self ? 1 : 0);
+    }
+    InitRows r{};
+    r.n = n;
+    r.ns = (int32_t)S.size();
+    r.npad = k - r.ns;
+    r.ld = ld;
+    r.s0 = pad_seed ? pad_seed : 0x9E3779B97F4A7C15ULL;
+    std::vector<uint64_t> tabs;
+    if (r.npad > 0) r.njump = xs_jump_tables(n, tabs);
+    CU(cudaSetDevice(ctx->device));
+    if (int rd = drop_speculation(ctx)) return rd;
+    DevScratch ds;
+    unsigned *taken = nullptr, *seedcnt = nullptr, *colcnt = nullptr;
+    uint64_t *rawoff = nullptr;
+    unsigned short *raw = nullptr;
+    CU(ds.alloc(&taken, (size_t)n));
+    CU(ds.alloc(&seedcnt, (size_t)n));
+    CU(ds.alloc(&colcnt, (size_t)ld));
+    CU(ds.alloc(&rawoff, (size_t)n + 1));
+    CU(ds.alloc(&raw, (size_t)npairs));
+    const unsigned row_blocks = (unsigned)((n + 255) / 256);
+    if (npairs > 0) {
+        int32_t *dS = nullptr;
+        CU(ds.alloc(&dS, S.size()));
+        CU(cudaMemcpyAsync(dS, S.data(), sizeof(int32_t) * S.size(), cudaMemcpyHostToDevice, ctx->stream));
+        const unsigned seed_blocks = (unsigned)((r.ns + kInitWarps - 1) / kInitWarps);
+        CU(cudaMemsetAsync(taken, 0, sizeof(unsigned) * (size_t)n, ctx->stream));
+        initf_seed_pairs_kernel<false><<<seed_blocks, 32 * kInitWarps, 0, ctx->stream>>>(r.ns, dS, ctx->d_rowptr, ctx->d_col, include_self, taken, rawoff, raw);
+        CU(cudaGetLastError());
+        if (int rs = scan_counts(ctx, ds, taken, n, 0, rawoff)) return rs;
+        CU(cudaMemsetAsync(taken, 0, sizeof(unsigned) * (size_t)n, ctx->stream));
+        initf_seed_pairs_kernel<true><<<seed_blocks, 32 * kInitWarps, 0, ctx->stream>>>(r.ns, dS, ctx->d_rowptr, ctx->d_col, include_self, taken, rawoff, raw);
+        initf_seed_rows_kernel<<<(unsigned)((n + kInitWarps - 1) / kInitWarps), 32 * kInitWarps, 0, ctx->stream>>>(n, r.ns, rawoff, raw, seedcnt);
+        CU(cudaGetLastError());
+    } else {
+        CU(cudaMemsetAsync(seedcnt, 0, sizeof(unsigned) * (size_t)n, ctx->stream));
+    }
+    uint64_t *dtabs = nullptr;
+    if (r.npad > 0) {
+        CU(ds.alloc(&dtabs, tabs.size()));
+        CU(cudaMemcpyAsync(dtabs, tabs.data(), sizeof(uint64_t) * tabs.size(), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    r.tabs = dtabs;
+    r.rawoff = rawoff;
+    r.raw = raw;
+    r.seedcnt = seedcnt;
+    r.cnt = taken;                    // (the pair counts are no longer needed)
+    r.colcnt = colcnt;
+    initf_rows_kernel<false><<<row_blocks, 256, 0, ctx->stream>>>(r);
+    CU(cudaGetLastError());
+    const int b = ctx->cur;
+    unsigned long long used = 0;
+    if (ctx->sparse) {
+        uint64_t *woff = nullptr;
+        CU(ds.alloc(&woff, (size_t)n + 1));
+        if (int rs = scan_counts(ctx, ds, r.cnt, n, 1, woff)) return rs;
+        CU(cudaMemcpyAsync(&used, woff + n, sizeof(used), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        if (used > ctx->pool_cap8) return fail(ctx, BIGCLAM_ENOMEM, "bigclam_init_F: rows need %llu pool words, %llu available", used, (unsigned long long)ctx->pool_cap8);
+        invalidate_resets(ctx);
+        r.woff = woff;
+        r.hdr = ctx->d_hdr[b];
+        r.pool = ctx->d_pool[b];
+    } else {
+        CU(cudaMemsetAsync(ctx->d_F[b], 0, sizeof(double) * (size_t)n * ld, ctx->stream));
+        r.F = ctx->d_F[b];
+    }
+    CU(cudaMemsetAsync(colcnt, 0, sizeof(unsigned) * (size_t)ld, ctx->stream));
+    initf_rows_kernel<true><<<row_blocks, 256, 0, ctx->stream>>>(r);
+    initf_sumF_kernel<<<(unsigned)((ld + 127) / 128), 128, 0, ctx->stream>>>(colcnt, ld, ctx->d_sumF[b]);   // :105-106
+    CU(cudaGetLastError());
+    if (ctx->sparse) {
+        CU(cudaMemcpyAsync(ctx->d_pool_top + b, &used, sizeof(used), cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        ctx->dense_valid = false;
+        if (int rt = retile(ctx, used)) return rt;
+    }
+    // with peer replicas every row counts as changed again: the next step publishes all owned rows
+    if (ctx->d_changed != nullptr) CU(cudaMemsetAsync(ctx->d_changed, 1, (size_t)n, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    return BIGCLAM_OK;
+}
+
 // Downloads the sparse state (sparse context) or the dense F (dense context) for the two getters below.
 static int fetch_rows_host(bigclam_ctx *ctx, std::vector<uint64_t> &hdr, std::vector<double> &pool, std::vector<double> &dense) {
     const int64_t n = ctx->n;
@@ -2495,6 +2650,11 @@ extern "C" int bigclam_multi_set_F(bigclam_multi *m, const double *F) {
 extern "C" int bigclam_multi_set_F_csr(bigclam_multi *m, const int64_t *indptr, const int32_t *indices, const double *values) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     for (bigclam_ctx *c : m->r) MCALL(bigclam_set_F_csr(c, indptr, indices, values), c);
+    return BIGCLAM_OK;
+}
+extern "C" int bigclam_multi_init_F(bigclam_multi *m, const int32_t *ranked_seeds, int64_t n_ranked, int32_t include_self, uint64_t pad_seed) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    for (bigclam_ctx *c : m->r) MCALL(bigclam_init_F(c, ranked_seeds, n_ranked, include_self, pad_seed), c);
     return BIGCLAM_OK;
 }
 extern "C" int bigclam_multi_set_sumF(bigclam_multi *m, const double *sumF) {

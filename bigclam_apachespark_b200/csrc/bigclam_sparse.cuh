@@ -1769,4 +1769,224 @@ __global__ void fold_bound_kernel(RowSrc s, const int64_t *__restrict__ rowptr, 
     if (lane == 0) bound[i] = t < s.k ? t : s.k;
 }
 
+// ------------------------------------------------------------------------------------------------
+// initNeighborComF(K) (bigclam4-7.scala:81-108) built as rows on the device (bigclam_init_F), bit for bit the n x K F0
+// of the host (bigclam_init_neighbor_com_F, initf.cpp) without ever holding it.  S = the selected seeds in id order:
+//   * column c < |S| is 1.0 on every entry of S[c]'s own neighbour list (and on S[c] with include_self): the pairs
+//     (row, c) are scattered from the seeds' lists (the CSR need not be symmetric; repeated entries and seeds allowed),
+//     then each row's columns are de-duplicated and sorted through a bitmap of |S| bits;
+//   * column c >= |S| is bit 33 of xorshift64*'s output for draw m = (c - |S|) n + u, i.e. of state s_(m+1).  The state
+//     update T is linear over GF(2): row u starts from T^(u+1) s_0 (byte tables of T^(2^j)) and moves from one padding
+//     column to the next with T^n, so every row draws exactly the host's bits, in ascending column order.
+// Counts and offsets come before anything is written (the pool check), and offsets are exclusive scans of the counts
+// in row order: the layout and pool_top follow from the rows alone.
+
+constexpr uint64_t kXsMul = 2685821657736338717ULL;   // xorshift64* output multiplier (initf.cpp)
+constexpr int kGf2Tab = 8 * 256;                      // byte tables of one 64 x 64 GF(2) matrix
+
+__host__ __device__ inline uint64_t xs_next(uint64_t s) {
+    s ^= s >> 12;
+    s ^= s << 25;
+    s ^= s >> 27;
+    return s;
+}
+__host__ __device__ inline uint64_t gf2_apply(const uint64_t *tab, uint64_t v) {
+    uint64_t r = 0;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) r ^= tab[b * 256 + (int)((v >> (8 * b)) & 255u)];
+    return r;
+}
+
+// (row, column) pairs of the seeds' lists, one warp per seed: counted per row (kScatter = false), then written to the
+// row's segment of raw (taken[] zeroed again in between).
+template <bool kScatter>
+__global__ void initf_seed_pairs_kernel(int ns, const int32_t *__restrict__ S, const int64_t *__restrict__ rowptr,
+                                        const int32_t *__restrict__ col, int include_self, unsigned *taken,
+                                        const uint64_t *__restrict__ rawoff, unsigned short *raw) {
+    const int lane = threadIdx.x & 31;
+    const int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (c >= ns) return;
+    const int32_t s = S[c];
+    const int64_t e0 = rowptr[s], e1 = rowptr[s + 1];
+    for (int64_t e = e0 + lane; e < e1 + (include_self ? 1 : 0); e += 32) {
+        const int32_t v = e < e1 ? col[e] : s;
+        const unsigned q = atomicAdd(taken + v, 1u);
+        if constexpr (kScatter) raw[rawoff[v] + q] = (unsigned short)c;
+    }
+}
+
+// One warp per row: its seed columns de-duplicated and ascending, written back to the front of its segment of raw.
+constexpr int kInitWarps = 8;
+__global__ void initf_seed_rows_kernel(int64_t n, int ns, const uint64_t *__restrict__ rawoff, unsigned short *raw,
+                                       unsigned *seedcnt) {
+    __shared__ unsigned bm_all[kInitWarps][kSpMaxK / 32];
+    __shared__ unsigned part_all[kInitWarps][32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int64_t u = (int64_t)blockIdx.x * kInitWarps + w;
+    if (u >= n) return;
+    const uint64_t e0 = rawoff[u], e1 = rawoff[u + 1];
+    if (e0 == e1) {
+        if (lane == 0) seedcnt[u] = 0;
+        return;
+    }
+    unsigned *bm = bm_all[w], *part = part_all[w];
+    const int nw = (ns + 31) >> 5, per = (nw + 31) >> 5;
+    for (int i = lane; i < nw; i += 32) bm[i] = 0u;
+    __syncwarp();
+    for (uint64_t e = e0 + lane; e < e1; e += 32) atomicOr(bm + (raw[e] >> 5), 1u << (raw[e] & 31));
+    __syncwarp();
+    const int w0 = min(nw, lane * per), w1 = min(nw, w0 + per);   // lane's words
+    unsigned mine = 0;
+    for (int i = w0; i < w1; ++i) mine += (unsigned)__popc(bm[i]);
+    part[lane] = mine;
+    __syncwarp();
+    unsigned q = 0, tot = 0;
+    for (int i = 0; i < 32; ++i) {
+        q += i < lane ? part[i] : 0u;
+        tot += part[i];
+    }
+    for (int i = w0; i < w1; ++i)
+        for (unsigned x = bm[i]; x != 0u; x &= x - 1u) raw[e0 + q++] = (unsigned short)(i * 32 + __ffs(x) - 1);
+    if (lane == 0) seedcnt[u] = tot;
+}
+
+struct InitRows {
+    int64_t n;
+    int32_t ns, npad, ld, njump;
+    uint64_t s0;                        // the padding sequence's seed state
+    const uint64_t *tabs;               // xs_jump_tables
+    const uint64_t *rawoff;             // n + 1
+    const unsigned short *raw;          // the rows' seed columns (initf_seed_rows_kernel)
+    const unsigned *seedcnt;            // n
+    unsigned *cnt;                      // n: written by the count pass, read by the fill pass
+    const uint64_t *woff;               // sparse rows: n + 1, the exclusive scan of sp_words(cnt)
+    uint64_t *hdr;
+    double *pool;
+    double *F;                          // dense rows (ld stride), zeroed before the fill pass
+    unsigned *colcnt;                   // ld, zeroed: the column counts (fill pass)
+};
+
+// One thread per row: the seed columns, then the padding bits.  The count pass (kFill = false) counts the row; the
+// fill pass writes it and adds its entries to the column counts.  Every thread of a block runs the padding loop
+// (the column counts are taken per warp).
+template <bool kFill>
+__global__ void initf_rows_kernel(InitRows r) {
+    __shared__ uint64_t stride_tab[kGf2Tab];
+    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = u < r.n;
+    if (r.npad > 0) {
+        for (int i = threadIdx.x; i < kGf2Tab; i += blockDim.x) stride_tab[i] = r.tabs[(size_t)r.njump * kGf2Tab + i];
+        __syncthreads();
+    }
+    const unsigned nseed = live ? r.seedcnt[u] : 0u;
+    double *ov = nullptr, *frow = nullptr;
+    unsigned short *oi = nullptr;
+    unsigned q = 0;
+    if (kFill && live) {
+        if (r.F != nullptr) {
+            frow = r.F + (size_t)u * r.ld;
+        } else {
+            const unsigned cnt = r.cnt[u];
+            const uint64_t off = r.woff[u];
+            ov = r.pool + off;
+            oi = sp_idx(ov, cnt);
+            for (unsigned i = cnt; i < sp_vpad(cnt); ++i) ov[i] = 0.0;
+            for (unsigned i = cnt; i < sp_ipad(cnt); ++i) oi[i] = 0;
+            r.hdr[u] = sp_pack(cnt ? off : 0, cnt);
+        }
+        const unsigned short *sc = r.raw + (live && nseed ? r.rawoff[u] : 0);
+        for (unsigned i = 0; i < nseed; ++i) {
+            const int c = sc[i];
+            if (frow != nullptr) frow[c] = 1.0;
+            else { ov[q] = 1.0; oi[q] = (unsigned short)c; ++q; }
+            atomicAdd(r.colcnt + c, 1u);
+        }
+    }
+    unsigned npad_set = 0;
+    if (r.npad > 0) {
+        uint64_t s = r.s0;
+        const uint64_t v = live ? (uint64_t)u + 1 : 0;
+        for (int j = 0; j < r.njump; ++j)
+            if ((v >> j) & 1u) s = gf2_apply(r.tabs + (size_t)j * kGf2Tab, s);
+        const int lane = threadIdx.x & 31;
+#pragma unroll 1
+        for (int j = 0; j < r.npad; ++j) {                  // s = state s_(j n + u + 1)
+            const bool bit = live && (((s * kXsMul) >> 33) & 1u);
+            npad_set += bit ? 1u : 0u;
+            if constexpr (kFill) {
+                const int c = r.ns + j;
+                if (bit) {
+                    if (frow != nullptr) frow[c] = 1.0;
+                    else { ov[q] = 1.0; oi[q] = (unsigned short)c; ++q; }
+                }
+                const unsigned b = __ballot_sync(0xffffffffu, bit);
+                if (lane == 0 && b != 0u) atomicAdd(r.colcnt + c, (unsigned)__popc(b));
+            }
+            s = gf2_apply(stride_tab, s);
+        }
+    }
+    if (!kFill && live) r.cnt[u] = nseed + npad_set;
+}
+
+__global__ void initf_sumF_kernel(const unsigned *__restrict__ colcnt, int ld, double *sumF) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c < ld) sumF[c] = (double)colcnt[c];
+}
+
+// Exclusive scan of n counts (or of sp_words(count)) into out[0 .. n], out[n] = the total: chunk sums, a scan of the
+// chunk sums in one block, then each chunk with its base.
+constexpr int kScanThreads = 256, kScanChunk = 4 * kScanThreads;
+__device__ inline uint64_t block_exclusive_scan(uint64_t x, uint64_t *sh, uint64_t *total) {
+    const int t = threadIdx.x;
+    sh[t] = x;
+    __syncthreads();
+    for (int off = 1; off < kScanThreads; off <<= 1) {
+        const uint64_t y = t >= off ? sh[t - off] : 0;
+        __syncthreads();
+        sh[t] += y;
+        __syncthreads();
+    }
+    const uint64_t incl = sh[t];
+    *total = sh[kScanThreads - 1];
+    __syncthreads();
+    return incl - x;
+}
+__device__ inline uint64_t scan_item(const unsigned *cnt, int64_t n, int words, int64_t i) {
+    if (i >= n) return 0;
+    return words ? sp_words(cnt[i]) : (uint64_t)cnt[i];
+}
+__global__ void scan_chunks_kernel(const unsigned *__restrict__ cnt, int64_t n, int words, uint64_t *chunk_sum) {
+    __shared__ uint64_t sh[kScanThreads];
+    const int64_t i0 = (int64_t)blockIdx.x * kScanChunk + 4 * threadIdx.x;
+    uint64_t x = 0, total = 0;
+    for (int k = 0; k < 4; ++k) x += scan_item(cnt, n, words, i0 + k);
+    block_exclusive_scan(x, sh, &total);
+    if (threadIdx.x == 0) chunk_sum[blockIdx.x] = total;
+}
+__global__ void scan_top_kernel(uint64_t *chunk_sum, int64_t nchunks, uint64_t *grand_total) {
+    __shared__ uint64_t sh[kScanThreads];
+    uint64_t carry = 0;
+    for (int64_t b0 = 0; b0 < nchunks; b0 += kScanThreads) {
+        const int64_t i = b0 + threadIdx.x;
+        const uint64_t x = i < nchunks ? chunk_sum[i] : 0;
+        uint64_t total = 0;
+        const uint64_t ex = block_exclusive_scan(x, sh, &total);
+        if (i < nchunks) chunk_sum[i] = carry + ex;
+        carry += total;
+    }
+    if (threadIdx.x == 0) *grand_total = carry;
+}
+__global__ void scan_apply_kernel(const unsigned *__restrict__ cnt, int64_t n, int words, const uint64_t *__restrict__ chunk_base,
+                                  uint64_t *out) {
+    __shared__ uint64_t sh[kScanThreads];
+    const int64_t i0 = (int64_t)blockIdx.x * kScanChunk + 4 * threadIdx.x;
+    uint64_t v[4], x = 0, total = 0;
+    for (int k = 0; k < 4; ++k) { v[k] = scan_item(cnt, n, words, i0 + k); x += v[k]; }
+    uint64_t p = chunk_base[blockIdx.x] + block_exclusive_scan(x, sh, &total);
+    for (int k = 0; k < 4; ++k) {
+        if (i0 + k < n) out[i0 + k] = p;
+        p += v[k];
+    }
+}
+
 }  // namespace bigclam

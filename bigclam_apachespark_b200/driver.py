@@ -262,18 +262,25 @@ class BigClam:
         self.conductance = cond
         return self.Sbc
 
-    def initNeighborComF(self, K: int, include_self: bool = False, pad_seed: int = 1234):
-        """Builds F0 from the ranked seeds and loads it (sets F and sumF like the script, :105-107)."""
+    def init_F(self, K: int, include_self: bool = False, pad_seed: int = 1234):
+        """initNeighborComF(K) (:81-108) built on the GPU, straight into the context: the F and sumF bits that loading
+        the host's n x K F0 gives (:105-107), with nothing n x K allocated on either side.  (Re)creates the context when
+        K changes and ranks the seeds (conductanceLocalMin) when that has not been done."""
         if getattr(self, "Sbc", None) is None:
             self.conductanceLocalMin()
-        F0 = np.empty((self.n, int(K)), dtype=np.float64)
-        rc = _lib.load().bigclam_init_neighbor_com_F(self.n, self.rowptr.ctypes.data, self.col.ctypes.data, int(K),
-                                                     self.Sbc.ctypes.data, len(self.Sbc), 1 if include_self else 0,
-                                                     C.c_uint64(pad_seed), F0.ctypes.data)
-        if rc != _lib.OK:
-            raise _lib.BigclamError(rc, "bigclam_init_neighbor_com_F failed")
-        self.set_F(F0)
-        return F0
+        if (self._ctx is None and self._multi is None) or int(K) != self.K:
+            self.set_K(int(K))
+        seeds = np.ascontiguousarray(self.Sbc, dtype=np.int32)
+        args = (seeds.ctypes.data, len(seeds), 1 if include_self else 0, C.c_uint64(pad_seed))
+        if self._multi is not None:
+            self._mcheck(_lib.load().bigclam_multi_init_F(self._multi, *args))
+        else:
+            check(_lib.load().bigclam_init_F(self._ctx, *args), self._ctx)
+        return self
+
+    def initNeighborComF(self, K: int, include_self: bool = False, pad_seed: int = 1234):
+        """Builds F0 from the ranked seeds and loads it (sets F and sumF like the script, :105-107); returns F0 (n x K)."""
+        return self.init_F(K, include_self, pad_seed).F
 
     # ---- the hot path ----
     def backtrackingLineSearchs(self, uset=None) -> float:
@@ -340,13 +347,13 @@ class BigClam:
         return Kset(self.minCom, self.maxCom, self.divCom)
 
     def sweep_K(self, rel_gain: float = 0.001, max_outer: int = 0):
-        """The K sweep at the bottom of the script (bigclam4-7.scala:244-266): for K in Kset, initNeighborComF(K),
+        """The K sweep at the bottom of the script (bigclam4-7.scala:244-266): for K in Kset, initNeighborComF(K) (init_F),
         SGDFindC(); stop at the first K whose LLH gain over the previous K is below 0.1 % (`1 - new/old < 0.001`).
         As coded, LLHKold starts at 0.0 (the `== null` test is never true for a Double), so the first K never
         stops the sweep.  Returns (KforC, [(K, LLH), ...]); KforC is 0 when the sweep ran out of K values (:245)."""
         LLHKold, KforC, hist = 0.0, 0, []
         for i in self.Kset():
-            self.initNeighborComF(i)
+            self.init_F(i)
             LLHKnew = self.SGDFindC(max_outer=max_outer)
             if self.verbose:
                 print(str(i) + " LLH: " + repr(LLHKnew))                                   # :258

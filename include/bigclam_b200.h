@@ -426,6 +426,17 @@ int bigclam_conductance_seeds_gpu(int64_t n, const int64_t *rowptr, const int32_
 int bigclam_init_neighbor_com_F(int64_t n, const int64_t *rowptr, const int32_t *col, int32_t k,
                                 const int32_t *ranked_seeds, int64_t n_ranked, int32_t include_self,
                                 uint64_t pad_seed, double *F_out);
+/*
+ * bigclam_init_F = initNeighborComF(K) (bigclam4-7.scala:81-108) built on the context's device, straight into the
+ * context, from the graph it was created with: the F rows and sumF bits that bigclam_init_neighbor_com_F(n, rowptr, col,
+ * K, ranked_seeds, n_ranked, include_self, pad_seed, F0) followed by bigclam_set_F(ctx, F0) leave, padding draws
+ * included, without an n x K array on either side (device scratch O(nnz(F0) + n + K)).  Column c of the first
+ * min(K, n_ranked) seeds in id order marks the entries of that seed's own neighbour list (any CSR: repeated entries and
+ * seeds allowed).  A seed outside [0, n) gives BIGCLAM_EINVAL, rows that do not fit the row pool BIGCLAM_ENOMEM; either
+ * way F and sumF stay as they were.  bigclam_multi_init_F builds the same rows on every rank.
+ */
+int bigclam_init_F(bigclam_ctx *ctx, const int32_t *ranked_seeds, int64_t n_ranked, int32_t include_self, uint64_t pad_seed);
+int bigclam_multi_init_F(bigclam_multi *m, const int32_t *ranked_seeds, int64_t n_ranked, int32_t include_self, uint64_t pad_seed);
 
 /* Library / device probe (no compute): returns the number of visible CUDA devices or <0. */
 int bigclam_device_count(void);

@@ -161,16 +161,20 @@ public:
         Sbc.resize((size_t)cnt);
         return Sbc;
     }
-    // initNeighborComF(K) (:81-108): builds F0 from the ranked seeds and loads it.
-    std::vector<double> initNeighborComF(int K, bool include_self = false, uint64_t pad_seed = 1234) {
+    // initNeighborComF(K) (:81-108) built on the device, straight into the context: the F and sumF bits that loading
+    // the host's n x K F0 gives (:105-107), with nothing n x K allocated on either side.
+    BigClam &init_F(int K, bool include_self = false, uint64_t pad_seed = 1234) {
         if (Sbc.empty()) conductanceLocalMin();
         if (K != K_ || (ctx_ == nullptr && multi_ == nullptr)) set_K(K);
-        std::vector<double> F0((size_t)(n_ * K));
-        const int rc = bigclam_init_neighbor_com_F(n_, rowptr_.data(), col_.data(), K, Sbc.data(), (int64_t)Sbc.size(), include_self ? 1 : 0,
-                                                   pad_seed, F0.data());
-        if (rc != BIGCLAM_OK) throw Error(rc, "bigclam_init_neighbor_com_F failed");
-        set_F(F0);
-        return F0;
+        const int32_t inc = include_self ? 1 : 0;
+        check(multi_ ? bigclam_multi_init_F(multi_, Sbc.data(), (int64_t)Sbc.size(), inc, pad_seed)
+                     : bigclam_init_F(ctx_, Sbc.data(), (int64_t)Sbc.size(), inc, pad_seed), "init_F");
+        return *this;
+    }
+    // initNeighborComF(K) (:81-108): builds F0 from the ranked seeds, loads it and returns it (n x K).
+    std::vector<double> initNeighborComF(int K, bool include_self = false, uint64_t pad_seed = 1234) {
+        init_F(K, include_self, pad_seed);
+        return F();
     }
 
     // ---- the hot path (:152-223).  uset: nullptr = all vertices (what the script always passes, :227)
@@ -305,13 +309,13 @@ public:
     }
 
     std::vector<int> Kset() const { return bigclam::Kset(minCom, maxCom, divCom); }
-    // The K sweep (:244-266): for K in Kset: initNeighborComF(K), SGDFindC(); stops at the first K whose gain
+    // The K sweep (:244-266): for K in Kset: initNeighborComF(K) (init_F), SGDFindC(); stops at the first K whose gain
     // `1 - new/old` is below 0.1 %.  As coded LLHKold starts at 0.0, so the first K never stops the sweep.
     // Returns KforC (0 when the grid ran out, :245) and fills hist with (K, LLH).
     int sweep_K(std::vector<std::pair<int, double>> *hist = nullptr, double rel_gain = 0.001, int64_t max_outer = 0) {
         double LLHKold = 0.0;
         for (int k : Kset()) {
-            initNeighborComF(k);
+            init_F(k);
             const double LLHKnew = SGDFindC(1e-4, max_outer);
             if (hist != nullptr) hist->emplace_back(k, LLHKnew);
             if (1.0 - LLHKnew / LLHKold < rel_gain) return k;          // (x / 0.0 = -inf or nan: never below, like the JVM)
