@@ -247,6 +247,13 @@ __device__ __forceinline__ double clamp_step0(double f, double s, double g, doub
     return (x > hi) ? hi : x;
 }
 
+// clamp_step of the column pair (2q, 2q + 1) of a dense row.  The padding columns k .. ld - 1 stay 0: with MIN_F_ > 0
+// clamp_step would lift them to MIN_F_, and they would enter the candidate's sums, the row and sumF.
+__device__ __forceinline__ double2 clamp_step2(double2 f, double s, double2 g, double lo, double hi, int q, int k) {
+    return make_double2((2 * q < k) ? clamp_step(f.x, s, g.x, lo, hi) : 0.0,
+                        (2 * q + 1 < k) ? clamp_step(f.y, s, g.y, lo, hi) : 0.0);
+}
+
 // Lower clamp only (used when no active component of the node can reach MAX_F_ at step 1).
 __device__ __forceinline__ double clamp_step0_lo(double f, double s, double g) {
     const double x = __dadd_rn(f, __dmul_rn(s, g));
@@ -514,7 +521,7 @@ __device__ __forceinline__ double ls_edge_range(const double *__restrict__ F, co
 // which it owns and overwrites afterwards) so that no register array has its address taken.
 template <int C2, int R>
 __device__ __noinline__ int dense_linesearch(const double *__restrict__ F, const int32_t *__restrict__ colp,
-                                             int ld, int nsteps, const double *s_steps, double alpha,
+                                             int k, int ld, int nsteps, const double *s_steps, double alpha,
                                              double min_f, double max_f, EdgeConst ec,
                                              const double *frow, const double *grow,
                                              const double *s_sumF, int deg, int lane,
@@ -532,8 +539,7 @@ __device__ __noinline__ int dense_linesearch(const double *__restrict__ F, const
                 const double2 sf = *reinterpret_cast<const double2 *>(s_sumF + 2 * q);
                 const double2 fu = ldg2(frow + 2 * q);
                 const double2 g = *reinterpret_cast<const double2 *>(grow + 2 * q);
-                nf[c].x = clamp_step(fu.x, s, g.x, min_f, max_f);
-                nf[c].y = clamp_step(fu.y, s, g.y, min_f, max_f);
+                nf[c] = clamp_step2(fu, s, g, min_f, max_f, q, k);
                 oa = fma(nf[c].x, (sf.x - fu.x) + nf[c].x, oa);
                 oa = fma(nf[c].y, (sf.y - fu.y) + nf[c].y, oa);
                 ob = fma(nf[c].x, nf[c].x, ob);
@@ -597,7 +603,7 @@ struct HubArgs {
     const HubItem *items;
     double *scratch;            // per mega hub: G[ld] | S1 | ST[16] | pad  (stride ld + 32 doubles)
     unsigned int *counters;     // per mega hub: [phase-1 slices done, phase-2 slices done]
-    int32_t n_peers, n_items, ld, nsteps, do_linesearch;
+    int32_t n_peers, n_items, k, ld, nsteps, do_linesearch;
     double alpha, min_f, max_f;
 };
 
@@ -866,7 +872,7 @@ __device__ __noinline__ void hub_phase(const HubArgs ha, const EdgeConst ec, con
                         if (q < ld2) *reinterpret_cast<double2 *>(orow + 2 * q) = g[c];
                     }
                     __syncwarp();
-                    const int jd = dense_linesearch<C2, 4>(F, colp, ld, ha.nsteps, s_steps, ha.alpha, ha.min_f, max_f, ec,
+                    const int jd = dense_linesearch<C2, 4>(F, colp, ha.k, ld, ha.nsteps, s_steps, ha.alpha, ha.min_f, max_f, ec,
                                                             F + (size_t)u * ld, orow, s_sumF, deg, lane, llh_u, G2);
                     if (lane == 0) hub_j[0] = jd;
                 }
@@ -895,8 +901,7 @@ __device__ __noinline__ void hub_phase(const HubArgs ha, const EdgeConst ec, con
                     if (q < ld2) {
                         double2 nr = fu[c];
                         if (jstar >= 0) {
-                            nr.x = clamp_step(fu[c].x, s, g[c].x, ha.min_f, max_f);
-                            nr.y = clamp_step(fu[c].y, s, g[c].y, ha.min_f, max_f);
+                            nr = clamp_step2(fu[c], s, g[c], ha.min_f, max_f, q, ha.k);
                             double2 *pd = reinterpret_cast<double2 *>(s_D + 2 * q);
                             double2 vd = *pd;
                             vd.x += fu[c].x - nr.x;
@@ -966,7 +971,7 @@ __global__ void __launch_bounds__(kBlockThreads, (C2 <= 4) ? 2 : 1) step_kernel(
             ha.accepted = a.accepted; ha.changed = a.changed;
             for (int r = 0; r < 7; ++r) ha.peer_out[r] = a.peer_out[r];
             ha.items = a.hub_items; ha.scratch = a.hub_scratch; ha.counters = a.hub_counters;
-            ha.n_peers = a.n_peers; ha.n_items = a.n_hub_items; ha.ld = ld; ha.nsteps = nsteps; ha.do_linesearch = a.do_linesearch;
+            ha.n_peers = a.n_peers; ha.n_items = a.n_hub_items; ha.k = a.k; ha.ld = ld; ha.nsteps = nsteps; ha.do_linesearch = a.do_linesearch;
             ha.alpha = a.alpha; ha.min_f = a.min_f; ha.max_f = max_f;
             double hub_llh = 0.0, hub_nupd = 0.0;
             hub_phase<C2>(ha, ec, s_sumF, s_steps, s_D, s_sumF + (size_t)ld * (1 + kWarpsPerBlock), lists, hub_small, &hub_llh, &hub_nupd);
@@ -1182,7 +1187,7 @@ __global__ void __launch_bounds__(kBlockThreads, (C2 <= 4) ? 2 : 1) step_kernel(
                     if (q < ld2) *reinterpret_cast<double2 *>(orow + 2 * q) = g[c];
                 }
                 __syncwarp();
-                jstar = dense_linesearch<C2, R>(F, a.col + e0, ld, nsteps, s_steps, a.alpha, a.min_f, max_f, ec,
+                jstar = dense_linesearch<C2, R>(F, a.col + e0, a.k, ld, nsteps, s_steps, a.alpha, a.min_f, max_f, ec,
                                                 F + (size_t)u * ld, orow, s_sumF, deg, lane, llh_u, G2);
             }
         }
@@ -1196,9 +1201,7 @@ __global__ void __launch_bounds__(kBlockThreads, (C2 <= 4) ? 2 : 1) step_kernel(
             for (int c = 0; c < C2; ++c) {
                 const int q = lane + 32 * c;
                 if (q < ld2) {
-                    double2 nr;
-                    nr.x = clamp_step(fu[c].x, s, g[c].x, a.min_f, max_f);
-                    nr.y = clamp_step(fu[c].y, s, g[c].y, a.min_f, max_f);
+                    const double2 nr = clamp_step2(fu[c], s, g[c], a.min_f, max_f, q, a.k);
                     *reinterpret_cast<double2 *>(orow + 2 * q) = nr;
                     double2 *pd = reinterpret_cast<double2 *>(s_D + 2 * q);
                     double2 vd = *pd;

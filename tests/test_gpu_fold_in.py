@@ -90,13 +90,14 @@ def _oracle_fold(O, rp, col, F, sumF, params, lst, max_iter, rel_tol):
     return f, l, it, tie
 
 
-def _check_against_oracle(b, rp, col, qrp, qcol, max_iter, rel_tol):
+def _check_against_oracle(b, rp, col, qrp, qcol, max_iter, rel_tol, params=None):
     """Every node agrees with the oracle loop (iters equal, same support, rows to 1e-12, llh to 1e-10) or its run went
     through a rounding-level Armijo tie; a node that has converged meets one at every further line search, so ties are
-    bounded only loosely."""
+    bounded only loosely.  params: the oracle's parameters, those of the context (default: the script's)."""
     from oracle import oracle as O
     F, sumF = b.F, b.sumF
-    params = O.make_params(b.K)
+    if params is None:
+        params = O.make_params(b.K)
     ip, ix, vl, llh, iters = b.fold_in(qrp, qcol, max_iter=max_iter, rel_tol=rel_tol)
     q = len(qrp) - 1
     assert ip.shape == (q + 1,) and ip[0] == 0 and (np.diff(ip) >= 0).all()
