@@ -2353,8 +2353,9 @@ static int extract_args_check(bigclam_ctx *ctx, const char *what, double delta, 
     return BIGCLAM_OK;
 }
 
-// The count pass: ptr (host, k + 2 entries) = the exclusive scan of the column sizes, column k being the zero rows.
-static int extract_count(bigclam_ctx *ctx, const char *what, double delta, std::vector<int64_t> &ptr) {
+// The count pass: ptr (host, k + 2 entries) = the exclusive scan of the column sizes, column k being the zero rows;
+// fmax (device, n, optional) gets row_fmax.
+static int extract_count(bigclam_ctx *ctx, const char *what, double delta, std::vector<int64_t> &ptr, double *fmax = nullptr) {
     CU(cudaSetDevice(ctx->device));
     const int64_t n = ctx->n;
     const int32_t k = ctx->p.k;
@@ -2367,7 +2368,7 @@ static int extract_count(bigclam_ctx *ctx, const char *what, double delta, std::
     CU(neg.reserve(1));
     CU(cudaMemsetAsync(ccnt.p, 0, sizeof(unsigned int) * ((size_t)k + 1), ctx->stream));
     CU(cudaMemsetAsync(neg.p, 0xff, sizeof(unsigned long long), ctx->stream));
-    colidx_kernel<false, MemberPred><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(row_src(ctx), n, MemberPred{delta, k, neg.p}, 0, k + 1,
+    colidx_kernel<false, MemberPred><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(row_src(ctx), n, MemberPred{delta, k, neg.p, fmax}, 0, k + 1,
                                                                                         ccnt.p, nullptr, nullptr);
     CU(cudaGetLastError());
     std::vector<unsigned int> hcnt((size_t)k + 1);
@@ -2444,6 +2445,47 @@ extern "C" int bigclam_extract_grouped(bigclam_ctx *ctx, double delta, int64_t *
             CU(cudaStreamSynchronize(ctx->stream));           // (hpos is reused by the next range)
         }
         c0 = c1;
+    }
+    return BIGCLAM_OK;
+}
+
+// Community scores (bigclam_b200.h, bigclam_community_stats): the count pass above gives |M_c|, z, row_fmax and the
+// F >= 0 check; community_stats_kernel the volumes and internal entries; the zero rows' part (zero_rows = 1) and the
+// conductance are added up here.
+extern "C" int bigclam_community_stats(bigclam_ctx *ctx, double delta, int32_t zero_rows, int64_t *size_out, int64_t *volume_out,
+                                       int64_t *internal_out, double *conductance_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_community_stats";
+    if (int rc = extract_args_check(ctx, what, delta, size_out, volume_out, internal_out)) return rc;
+    if (zero_rows != 0 && zero_rows != 1) return fail(ctx, BIGCLAM_EINVAL, "%s: zero_rows = %d, must be 0 or 1", what, zero_rows);
+    CU(cudaSetDevice(ctx->device));
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k;
+    std::vector<unsigned long long> h((size_t)2 * k + 2, 0ull);   // volume[k], internal[k], zero rows' degrees, entries between zero rows
+    std::vector<int64_t> ptr((size_t)k + 2, 0);
+    if (n > 0) {
+        DevBuf<double> fmax;
+        DevBuf<unsigned long long> cnt;
+        if (fmax.reserve((size_t)n) != cudaSuccess || cnt.reserve(h.size()) != cudaSuccess)
+            return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for %lld bytes of scratch", what, (long long)(8 * (n + (int64_t)h.size())));
+        if (int rc = extract_count(ctx, what, delta, ptr, fmax.p)) return rc;
+        CU(cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long) * h.size(), ctx->stream));
+        const size_t smem = sizeof(unsigned int) * (size_t)kStatWarps * (size_t)((k + 31) / 32);
+        community_stats_kernel<<<(unsigned)((n + kStatWarps - 1) / kStatWarps), 32 * kStatWarps, smem, ctx->stream>>>(
+            row_src(ctx), ctx->d_rowptr, ctx->d_col, n, fmax.p, delta, zero_rows == 1, cnt.p, cnt.p + k, cnt.p + 2 * k);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(h.data(), cnt.p, sizeof(unsigned long long) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    const bool z_in = zero_rows == 1;
+    const int64_t z = z_in ? ptr[(size_t)k + 1] - ptr[(size_t)k] : 0;
+    const int64_t zdeg = z_in ? (int64_t)h[2 * (size_t)k] : 0, zz = z_in ? (int64_t)h[2 * (size_t)k + 1] : 0;
+    for (int32_t c = 0; c < k; ++c) {
+        size_out[c] = ptr[(size_t)c + 1] - ptr[(size_t)c] + z;
+        volume_out[c] = (int64_t)h[(size_t)c] + zdeg;
+        internal_out[c] = (int64_t)h[(size_t)k + c] + zz;
+        if (conductance_out != nullptr)
+            conductance_out[c] = conductance_formula((double)(volume_out[c] - internal_out[c]), (double)internal_out[c], (double)ctx->nnz);
     }
     return BIGCLAM_OK;
 }
@@ -2725,6 +2767,13 @@ extern "C" int bigclam_multi_extract_nnz(bigclam_multi *m, double delta, int64_t
 extern "C" int bigclam_multi_extract_grouped(bigclam_multi *m, double delta, int64_t *comptr_out, int32_t *members_out, int32_t *zero_rows_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     MCALL(bigclam_extract_grouped(m->r[0], delta, comptr_out, members_out, zero_rows_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_multi_community_stats(bigclam_multi *m, double delta, int32_t zero_rows, int64_t *size_out, int64_t *volume_out,
+                                             int64_t *internal_out, double *conductance_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_community_stats(m->r[0], delta, zero_rows, size_out, volume_out, internal_out, conductance_out), m->r[0]);
     return BIGCLAM_OK;
 }
 

@@ -1434,6 +1434,7 @@ struct MemberPred {
     double delta;
     int k;
     unsigned long long *neg;
+    double *fmax = nullptr;            // (optional) fmax[u] = row_fmax, for community_stats_kernel
     struct Row {
         double fmax;
     };
@@ -1443,7 +1444,9 @@ struct MemberPred {
             for (int i = lane; i < r.cnt; i += 32) any |= r.vals[i] < 0.0;
             if (any) atomic_min_u64(neg, (unsigned long long)u);
         }
-        return Row{row_fmax(s, r, lane)};
+        const double mx = row_fmax(s, r, lane);
+        if (fmax != nullptr && lane == 0) fmax[u] = mx;
+        return Row{mx};
     }
     __device__ __forceinline__ bool take(const Row &st, double v) const { return is_member(v, st.fmax, delta); }
     __device__ __forceinline__ int whole(const Row &st) const { return st.fmax == 0.0 ? k : -1; }
@@ -1503,6 +1506,82 @@ __global__ void extract_rows_kernel(RowSrc s, int64_t r0, int64_t r1, double del
     }
     for (int i = lane; i < r.cnt; i += 32) m[r.idx != nullptr ? (int)r.idx[i] : i] = is_member(r.vals[i], mx, delta);
     if (lane == 0) fmax[u - r0] = mx;
+}
+
+// Community scores (bigclam_community_stats): volume[c] and internal[c] over the members M(u) of is_member, with
+// fmax[u] = row_fmax from the count pass (colidx_kernel with MemberPred, which also checks F >= 0); fmax 0 marks a zero
+// row, whose memberships are not walked.  One warp per row u, the lanes over u's list entries u -> v:
+//   u not a zero row  M(u) goes to the warp's bitmap of k bits in shared memory; volume[c] += deg(u) for c in M(u).  A lane
+//                     walks the stored entries of each v that is not a zero row: internal[c] += 1 for each c in M(v)
+//                     whose bit is set.  zero_rows: the entries to zero rows add their count to internal[c], c in M(u);
+//   u a zero row      (zero_rows only) internal[c] += 1 for c in M(v) of every entry to a v that is not a zero row;
+//                     scal[0] += deg(u) and scal[1] += the entries to zero rows, which the host adds to every c.
+// The work is O(entries x stored row length), never O(k x zero-row degree).
+constexpr int kStatWarps = 8;
+__global__ void community_stats_kernel(RowSrc s, const int64_t *__restrict__ rowptr, const int32_t *__restrict__ col, int64_t n,
+                                       const double *__restrict__ fmax, double delta, bool zero_rows,
+                                       unsigned long long *__restrict__ volume, unsigned long long *__restrict__ internal,
+                                       unsigned long long *__restrict__ scal) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31;
+    const int64_t u = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (u >= n) return;                                      // (warp-uniform)
+    const double fu = fmax[u];
+    const int64_t e0 = rowptr[u], e1 = rowptr[u + 1];
+    if (fu == 0.0) {
+        if (!zero_rows) return;
+        unsigned long long zz = 0;
+        for (int64_t e = e0 + lane; e < e1; e += 32) {
+            const int32_t v = col[e];
+            const double fv = fmax[v];
+            if (fv == 0.0) {
+                ++zz;
+                continue;
+            }
+            const RowView r = row_view(s, v);
+            for (int i = 0; i < r.cnt; ++i)
+                if (is_member(r.vals[i], fv, delta)) atomicAdd(&internal[r.idx != nullptr ? (int)r.idx[i] : i], 1ull);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) zz += __shfl_xor_sync(0xffffffffu, zz, o);
+        if (lane == 0) {
+            atomicAdd(&scal[0], (unsigned long long)(e1 - e0));
+            if (zz != 0) atomicAdd(&scal[1], zz);
+        }
+        return;
+    }
+    const int words = (s.k + 31) >> 5;
+    unsigned int *bits = reinterpret_cast<unsigned int *>(smem_raw) + (threadIdx.x >> 5) * words;
+    for (int i = lane; i < words; i += 32) bits[i] = 0u;
+    __syncwarp();
+    const RowView ru = row_view(s, u);
+    for (int i = lane; i < ru.cnt; i += 32)
+        if (is_member(ru.vals[i], fu, delta)) {
+            const int c = ru.idx != nullptr ? (int)ru.idx[i] : i;
+            atomicOr(&bits[c >> 5], 1u << (c & 31));
+            atomicAdd(&volume[c], (unsigned long long)(e1 - e0));
+        }
+    __syncwarp();
+    unsigned long long zn = 0;
+    for (int64_t e = e0 + lane; e < e1; e += 32) {
+        const int32_t v = col[e];
+        const double fv = fmax[v];
+        if (fv == 0.0) {
+            ++zn;
+            continue;
+        }
+        const RowView r = row_view(s, v);
+        for (int i = 0; i < r.cnt; ++i) {
+            const int c = r.idx != nullptr ? (int)r.idx[i] : i;
+            if (((bits[c >> 5] >> (c & 31)) & 1u) && is_member(r.vals[i], fv, delta)) atomicAdd(&internal[c], 1ull);
+        }
+    }
+    if (!zero_rows) return;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) zn += __shfl_xor_sync(0xffffffffu, zn, o);
+    if (zn == 0) return;                                     // (warp-uniform)
+    for (int i = lane; i < ru.cnt; i += 32)
+        if (is_member(ru.vals[i], fu, delta)) atomicAdd(&internal[ru.idx != nullptr ? (int)ru.idx[i] : i], zn);
 }
 
 struct SampleArgs {

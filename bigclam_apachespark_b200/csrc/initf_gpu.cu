@@ -51,9 +51,7 @@ __global__ void conductance_kernel(int64_t n, const int64_t *__restrict__ rowptr
         inside += __shfl_xor_sync(0xffffffffu, inside, o);
     }
     if (lane == 0) {
-        const double cut_S = (double)(zsize - inside), vol_S = (double)inside;      // :64-65
-        const double vol_T = sigma - vol_S - cut_S * 2;                             // :66
-        cond[x] = (vol_S == 0) ? 0.0 : (vol_T == 0) ? 1.0 : cut_S / fmin(vol_S, vol_T);   // :67
+        cond[x] = bigclam::conductance_formula((double)(zsize - inside), (double)inside, sigma);   // :64-67
     }
 }
 

@@ -477,6 +477,25 @@ class BigClam:
             check(lib.bigclam_extract_grouped(self._ctx, delta, *outs), self._ctx)
         return comptr, members[:nnz.value], zero_rows[:z.value]
 
+    def community_stats(self, delta, zero_rows_everywhere=True):
+        """A label-free score of every community of extract_communities(delta), on the GPU.  Returns dict(size, volume,
+        internal, conductance), arrays of length K: |S_c|; the sum of deg(u) over u in S_c; the neighbour-list entries
+        u -> v with u and v in S_c (entries counted with multiplicity, self loops included); and conductanceLocalMin's
+        formula (bigclam4-7.scala:64-67) with cut = volume - internal, vol_S = internal and sigma = the number of list
+        entries of the graph (an empty community scores 0).  zero_rows_everywhere: all-zero rows are in every community
+        (as coded) or in none, the two choices of communities.group()."""
+        lib = _lib.load()
+        K = self.K
+        size, volume, internal = (np.zeros(K, dtype=np.int64) for _ in range(3))
+        cond = np.zeros(K, dtype=np.float64)
+        args = (float(delta), 1 if zero_rows_everywhere else 0, size.ctypes.data, volume.ctypes.data, internal.ctypes.data,
+                cond.ctypes.data)
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_community_stats(self._multi, *args))
+        else:
+            check(lib.bigclam_community_stats(self._need(), *args), self._ctx)
+        return dict(size=size, volume=volume, internal=internal, conductance=cond)
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

@@ -312,6 +312,37 @@ int bigclam_multi_extract_nnz(bigclam_multi *m, double delta, int64_t *nnz_out, 
 int bigclam_multi_extract_grouped(bigclam_multi *m, double delta, int64_t *comptr_out, int32_t *members_out, int32_t *zero_rows_out);
 
 /*
+ * A score for every community of the current F, with no ground truth needed.  Membership is the rule above (delta > 0
+ * and not NaN, +inf allowed, else BIGCLAM_EINVAL before any device work; a negative entry gives BIGCLAM_EUNSUPPORTED
+ * naming the smallest such row).  As coded an all-zero row belongs to every community; zero_rows chooses:
+ *   1: the zero rows are in every community, as coded;   0: they are in no community;   anything else: BIGCLAM_EINVAL.
+ * With S_c the member set of community c and the graph the context was created with (deg(u) = rowptr[u + 1] - rowptr[u],
+ * list entries counted with their multiplicity, self-loop entries included; the graph need not be symmetric):
+ *   size_out[c]        = |S_c|
+ *   volume_out[c]      = sum over u in S_c of deg(u)
+ *   internal_out[c]    = the list entries u -> v with u and v in S_c (vol_S of bigclam4-7.scala:65; for a symmetric
+ *                        graph without repeated entries, twice the edges inside S_c).  The cut is volume - internal.
+ *   conductance_out[c] (optional) = conductanceLocalMin's formula (:64-67, bigclam::conductance_formula below) with
+ *                        cut_S = volume - internal, vol_S = internal, sigma = rowptr[n]:
+ *                        vol_T = sigma - vol_S - 2 cut_S;  0 if vol_S == 0, else 1 if vol_T == 0, else cut_S / min(vol_S, vol_T).
+ *                        So an empty community (and any community without an internal entry) scores 0, and on multigraph
+ *                        input vol_T, and with it the score, can be negative, as coded.  The textbook conductance is
+ *                        cut / min(volume, sigma - volume); it is not an output.
+ * An ego net scored this way equals conductanceLocalMin's score of its centre when the centre's own list has no repeated
+ * entry and no self loop: :63 walks a repeated neighbour's list once per repetition, a set walks it once.
+ *
+ * Output (k values each) depends on (F bits, delta, graph, zero_rows) only: not on the row layout, the number of GPUs
+ * or the device.  Device scratch is O(n + k), nothing n x k (BIGCLAM_ENOMEM when even that cannot be allocated).  Reads F
+ * only (no state changes: F, sumF, accepted indices, a speculative step), on the context's stream, synchronous.  A NULL
+ * required output gives BIGCLAM_EINVAL; n = 0 gives zeros.  The multi-GPU call reads rank 0's replica; its errors go to
+ * bigclam_multi_last_error.
+ */
+int bigclam_community_stats(bigclam_ctx *ctx, double delta, int32_t zero_rows, int64_t *size_out /* k */, int64_t *volume_out /* k */,
+                            int64_t *internal_out /* k */, double *conductance_out /* k, optional */);
+int bigclam_multi_community_stats(bigclam_multi *m, double delta, int32_t zero_rows, int64_t *size_out, int64_t *volume_out,
+                                  int64_t *internal_out, double *conductance_out);
+
+/*
  * The fitted model as a model of edges (the clamp of bigclam4-7.scala:166, the edge term of :218), on the current F:
  *   x_uv = sum of F_uc * F_vc over the components c that are non-zero in both rows, folded left in ascending c with
  *          every product and every sum rounded on its own (the same bits for sparse and dense rows and for (v, u));
@@ -444,5 +475,21 @@ const char *bigclam_version(void);
 
 #ifdef __cplusplus
 }
+
+#include <math.h>
+#if defined(__CUDACC__)
+#define BIGCLAM_HD __host__ __device__
+#else
+#define BIGCLAM_HD
+#endif
+namespace bigclam {
+/* The conductance of conductanceLocalMin (bigclam4-7.scala:64-67) from cut_S, vol_S and sigma (integers as doubles):
+ * the ego nets of bigclam_conductance_seeds_gpu and the communities of bigclam_community_stats score through it. */
+BIGCLAM_HD inline double conductance_formula(double cut_S, double vol_S, double sigma) {
+    const double vol_T = sigma - vol_S - cut_S * 2;                                   /* :66 */
+    return (vol_S == 0) ? 0.0 : (vol_T == 0) ? 1.0 : cut_S / fmin(vol_S, vol_T);    /* :67 */
+}
+}  // namespace bigclam
+#undef BIGCLAM_HD
 #endif
 #endif /* BIGCLAM_B200_H */

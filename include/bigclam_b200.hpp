@@ -17,6 +17,7 @@
 //   K sweep                                           :244-266   sweep_K()
 //   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta),
 //                                                                extract_grouped(delta, ...)
+//   community scores, the formula of conductanceLocalMin :64-67  community_stats(delta, zero_rows_everywhere)
 //   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m),
 //                                                                sample_graph(seed, eps)
 //   rows for new nodes, the fit held fixed (:157-184 per node)    fold_in(rowptr, col, max_iter, rel_tol, ...)
@@ -239,6 +240,28 @@ public:
               "extract");
         members.resize((size_t)nnz);
         zero_rows.resize((size_t)z);
+    }
+
+    // A label-free score of every community of extract(delta) (bigclam_community_stats): size |S_c|, volume (sum of deg(u)
+    // over S_c), internal (list entries u -> v with u, v in S_c; the cut is volume - internal) and conductanceLocalMin's
+    // formula of :64-67 on them.  zero_rows_everywhere: all-zero rows in every community (as coded) or in none.  Works
+    // for multi-GPU handles too.
+    struct CommunityStats {
+        std::vector<int64_t> size, volume, internal;
+        std::vector<double> conductance;
+    };
+    CommunityStats community_stats(double delta, bool zero_rows_everywhere = true) {
+        need();
+        CommunityStats s;
+        s.size.assign((size_t)K_, 0);
+        s.volume.assign((size_t)K_, 0);
+        s.internal.assign((size_t)K_, 0);
+        s.conductance.assign((size_t)K_, 0.0);
+        const int32_t zr = zero_rows_everywhere ? 1 : 0;
+        check(multi_ ? bigclam_multi_community_stats(multi_, delta, zr, s.size.data(), s.volume.data(), s.internal.data(), s.conductance.data())
+                     : bigclam_community_stats(ctx_, delta, zr, s.size.data(), s.volume.data(), s.internal.data(), s.conductance.data()),
+              "community_stats");
+        return s;
     }
 
     // The fitted model as a model of edges, P(u,v) = 1 - exp(-F_u.F_v) with the clamp of :166 (bigclam_pair_affinity):
