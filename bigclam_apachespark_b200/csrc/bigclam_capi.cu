@@ -2490,6 +2490,145 @@ extern "C" int bigclam_community_stats(bigclam_ctx *ctx, double delta, int32_t z
     return BIGCLAM_OK;
 }
 
+// Cover scores (bigclam_b200.h, bigclam_cover_scores).  The host checks the truth cover and keeps the first copy of each
+// id in a community (a stamp per node: O(n + sum |Y_t|)); the count pass gives |M_c|, z, row_fmax and the F >= 0 check;
+// cover_scores_kernel<false> the per-pair maxima and minima, <true> the detected side's matches; the means and sums
+// are folded here in ascending id.
+extern "C" int bigclam_cover_scores(bigclam_ctx *ctx, double delta, int32_t zero_rows, int64_t q, const int64_t *truth_ptr,
+                                    const int32_t *truth_members, double *f1_det, int32_t *match_det, double *f1_truth,
+                                    int32_t *match_truth, double *hcond_det, double *hcond_truth, double *scores_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_cover_scores";
+    if (!(delta > 0.0)) return fail(ctx, BIGCLAM_EINVAL, "%s: delta = %g, must be > 0", what, delta);
+    if (zero_rows != 0 && zero_rows != 1) return fail(ctx, BIGCLAM_EINVAL, "%s: zero_rows = %d, must be 0 or 1", what, zero_rows);
+    if (q < 0 || q > INT32_MAX) return fail(ctx, BIGCLAM_EINVAL, "%s: q = %lld, must be in [0, 2^31 - 1]", what, (long long)q);
+    if (f1_det == nullptr || match_det == nullptr || scores_out == nullptr || (q > 0 && (f1_truth == nullptr || match_truth == nullptr)))
+        return fail(ctx, BIGCLAM_EINVAL, "%s: NULL output", what);
+    if (truth_ptr == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: NULL truth_ptr", what);
+    if (truth_ptr[0] != 0) return fail(ctx, BIGCLAM_EINVAL, "%s: truth_ptr[0] = %lld, must be 0", what, (long long)truth_ptr[0]);
+    for (int64_t t = 0; t < q; ++t)
+        if (truth_ptr[t + 1] < truth_ptr[t])
+            return fail(ctx, BIGCLAM_EINVAL, "%s: truth_ptr decreases at truth community %lld", what, (long long)t);
+    if (truth_ptr[q] > 0 && truth_members == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: NULL truth_members", what);
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k;
+    std::vector<int32_t> stamp((size_t)n, -1);
+    std::vector<int64_t> tptr((size_t)q + 1, 0);
+    std::vector<int32_t> tmem;
+    tmem.reserve((size_t)truth_ptr[q]);
+    for (int64_t t = 0; t < q; ++t) {
+        for (int64_t i = truth_ptr[t]; i < truth_ptr[t + 1]; ++i) {
+            const int32_t u = truth_members[i];
+            if (u < 0 || u >= n)
+                return fail(ctx, BIGCLAM_EINVAL, "%s: truth community %lld has id %d outside [0, %lld)", what, (long long)t, u, (long long)n);
+            if (stamp[(size_t)u] != (int32_t)t) {
+                stamp[(size_t)u] = (int32_t)t;
+                tmem.push_back(u);
+            }
+        }
+        tptr[(size_t)t + 1] = (int64_t)tmem.size();
+    }
+    constexpr unsigned long long kInfBits = 0x7ff0000000000000ull;
+    std::vector<int64_t> ptr((size_t)k + 2, 0), xs((size_t)k, 0);
+    std::vector<unsigned long long> bits((size_t)2 * k);                 // f1_det bits from 0, hc_det bits from +inf
+    std::fill(bits.begin(), bits.begin() + k, 0ull);
+    std::fill(bits.begin() + k, bits.end(), kInfBits);
+    std::vector<unsigned int> md((size_t)k, ~0u);
+    std::vector<double> hx((size_t)k, NAN), tf((size_t)3 * q);          // per t: f1, hcond (+inf: none admissible), H(Y_t)
+    std::vector<int32_t> tm((size_t)q, -1);
+    if (n > 0) {
+        CU(cudaSetDevice(ctx->device));
+        const int64_t nm = (int64_t)tmem.size();
+        DevBuf<double> fmax, h, hs, dtf;
+        DevBuf<int64_t> dxs, dptr;
+        DevBuf<int32_t> dmem, dtm;
+        DevBuf<unsigned long long> dbits;
+        DevBuf<unsigned int> dmd;
+        if (fmax.reserve((size_t)n) != cudaSuccess || h.reserve((size_t)n + 1) != cudaSuccess || hs.reserve((size_t)k) != cudaSuccess ||
+            dtf.reserve((size_t)3 * q) != cudaSuccess || dxs.reserve((size_t)k) != cudaSuccess || dptr.reserve((size_t)q + 1) != cudaSuccess ||
+            dmem.reserve((size_t)nm) != cudaSuccess || dtm.reserve((size_t)q) != cudaSuccess || dbits.reserve((size_t)2 * k) != cudaSuccess ||
+            dmd.reserve((size_t)k) != cudaSuccess)
+            return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for %lld bytes of scratch", what,
+                        (long long)(8 * (2 * n + 1) + 36 * (int64_t)k + 36 * q + 8 + 4 * nm));
+        if (int rc = extract_count(ctx, what, delta, ptr, fmax.p)) return rc;
+        const int64_t z = zero_rows == 1 ? ptr[(size_t)k + 1] - ptr[(size_t)k] : 0;
+        for (int32_t c = 0; c < k; ++c) xs[(size_t)c] = ptr[(size_t)c + 1] - ptr[(size_t)c] + z;
+        CU(cudaMemcpyAsync(dxs.p, xs.data(), sizeof(int64_t) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dptr.p, tptr.data(), sizeof(int64_t) * ((size_t)q + 1), cudaMemcpyHostToDevice, ctx->stream));
+        if (nm > 0) CU(cudaMemcpyAsync(dmem.p, tmem.data(), sizeof(int32_t) * (size_t)nm, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dbits.p, bits.data(), sizeof(unsigned long long) * bits.size(), cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dmd.p, md.data(), sizeof(unsigned int) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
+        cover_h_kernel<<<(unsigned)((n + 256) / 256), 256, 0, ctx->stream>>>(n, h.p);
+        CU(cudaGetLastError());
+        cover_hsize_kernel<<<(unsigned)((k + 255) / 256), 256, 0, ctx->stream>>>(h.p, n, dxs.p, k, hs.p);
+        CU(cudaGetLastError());
+        if (q > 0) {
+            const size_t smem = sizeof(unsigned int) * (size_t)k;
+            CU(cudaFuncSetAttribute(cover_scores_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            CU(cudaFuncSetAttribute(cover_scores_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            const CoverArgs ca{row_src(ctx), fmax.p, dptr.p, dmem.p, dxs.p, h.p, n, delta, zero_rows == 1,
+                               dbits.p, dbits.p + k, dmd.p, dtf.p, dtf.p + q, dtf.p + 2 * q, dtm.p};
+            cover_scores_kernel<false><<<(unsigned)q, 32 * kCoverWarps, smem, ctx->stream>>>(ca);
+            CU(cudaGetLastError());
+            cover_scores_kernel<true><<<(unsigned)q, 32 * kCoverWarps, smem, ctx->stream>>>(ca);
+            CU(cudaGetLastError());
+            CU(cudaMemcpyAsync(tf.data(), dtf.p, sizeof(double) * tf.size(), cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaMemcpyAsync(tm.data(), dtm.p, sizeof(int32_t) * (size_t)q, cudaMemcpyDeviceToHost, ctx->stream));
+        }
+        CU(cudaMemcpyAsync(bits.data(), dbits.p, sizeof(unsigned long long) * bits.size(), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(md.data(), dmd.p, sizeof(unsigned int) * (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(hx.data(), hs.p, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    auto as_double = [](unsigned long long b) {
+        double d;
+        std::memcpy(&d, &b, sizeof d);
+        return d;
+    };
+    // left folds in ascending id: F1 over the non-empty communities; the NMI terms over those of size in (0, n)
+    double f1x = 0.0, f1y = 0.0, rx = 0.0, ry = 0.0, hx_sum = 0.0, hy_sum = 0.0, hcx_sum = 0.0, hcy_sum = 0.0;
+    int64_t nx = 0, nnx = 0, nny = 0;
+    for (int32_t c = 0; c < k; ++c) {
+        const int64_t x = xs[(size_t)c];
+        f1_det[c] = as_double(bits[(size_t)c]);
+        match_det[c] = bits[(size_t)c] != 0ull ? (int32_t)md[(size_t)c] : -1;
+        double hc = NAN;
+        if (x > 0 && x < n) {
+            const unsigned long long b = bits[(size_t)k + c];
+            hc = b == kInfBits ? hx[(size_t)c] : as_double(b);
+            rx += hc / hx[(size_t)c];
+            hx_sum += hx[(size_t)c];
+            hcx_sum += hc;
+            ++nnx;
+        }
+        if (hcond_det != nullptr) hcond_det[c] = hc;
+        if (x > 0) {
+            f1x += f1_det[c];
+            ++nx;
+        }
+    }
+    for (int64_t t = 0; t < q; ++t) {
+        const int64_t y = tptr[(size_t)t + 1] - tptr[(size_t)t];
+        f1_truth[t] = y > 0 ? tf[(size_t)t] : 0.0;
+        match_truth[t] = y > 0 ? tm[(size_t)t] : -1;
+        double hc = NAN;
+        if (y > 0 && y < n) {
+            const double hy = tf[(size_t)(2 * q + t)];
+            hc = std::isinf(tf[(size_t)(q + t)]) ? hy : tf[(size_t)(q + t)];
+            ry += hc / hy;
+            hy_sum += hy;
+            hcy_sum += hc;
+            ++nny;
+        }
+        if (hcond_truth != nullptr) hcond_truth[t] = hc;
+        f1y += f1_truth[t];
+    }
+    scores_out[0] = (nx == 0 || q == 0) ? 0.0 : 0.5 * (f1x / (double)nx + f1y / (double)q);
+    scores_out[1] = (nnx == 0 || nny == 0) ? NAN : 1.0 - 0.5 * (rx / (double)nnx + ry / (double)nny);
+    scores_out[2] = (nnx == 0 || nny == 0) ? NAN : 0.5 * ((hx_sum - hcx_sum) + (hy_sum - hcy_sum)) / std::max(hx_sum, hy_sum);
+    return BIGCLAM_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Fused collective of the node-partitioned path: exchange buffers (see bigclam_ctx::x_*).
 static int xchg_alloc(bigclam_ctx *ctx, int32_t world, int32_t rank) {
@@ -2774,6 +2913,16 @@ extern "C" int bigclam_multi_community_stats(bigclam_multi *m, double delta, int
                                              int64_t *internal_out, double *conductance_out) {
     if (m == nullptr) return BIGCLAM_EINVAL;
     MCALL(bigclam_community_stats(m->r[0], delta, zero_rows, size_out, volume_out, internal_out, conductance_out), m->r[0]);
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_multi_cover_scores(bigclam_multi *m, double delta, int32_t zero_rows, int64_t q, const int64_t *truth_ptr,
+                                          const int32_t *truth_members, double *f1_det, int32_t *match_det, double *f1_truth,
+                                          int32_t *match_truth, double *hcond_det, double *hcond_truth, double *scores_out) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    MCALL(bigclam_cover_scores(m->r[0], delta, zero_rows, q, truth_ptr, truth_members, f1_det, match_det, f1_truth, match_truth,
+                               hcond_det, hcond_truth, scores_out),
+          m->r[0]);
     return BIGCLAM_OK;
 }
 

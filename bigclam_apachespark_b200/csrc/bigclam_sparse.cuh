@@ -1408,14 +1408,20 @@ __device__ __forceinline__ double row_fmax(const RowSrc &s, const RowView &r, in
 }
 __host__ __device__ __forceinline__ bool is_member(double v, double fmax, double delta) { return fmax < delta ? v == fmax : v >= delta; }
 
-#ifdef BIGCLAM_EMU          // host emulation (tests/emu): no atomicMin there
-inline void atomic_min_u64(unsigned long long *p, unsigned long long v) {
-    unsigned long long old = __atomic_load_n(p, __ATOMIC_SEQ_CST);
-    while (v < old && !__atomic_compare_exchange_n(p, &old, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {
+#ifdef BIGCLAM_EMU          // host emulation (tests/emu): no atomicMin / atomicMax there
+template <bool kMax, class T>
+inline void atomic_extreme(T *p, T v) {
+    T old = __atomic_load_n(p, __ATOMIC_SEQ_CST);
+    while ((kMax ? v > old : v < old) && !__atomic_compare_exchange_n(p, &old, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {
     }
 }
+inline void atomic_min_u64(unsigned long long *p, unsigned long long v) { atomic_extreme<false>(p, v); }
+inline void atomic_max_u64(unsigned long long *p, unsigned long long v) { atomic_extreme<true>(p, v); }
+inline void atomic_min_u32(unsigned int *p, unsigned int v) { atomic_extreme<false>(p, v); }
 #else
 __device__ __forceinline__ void atomic_min_u64(unsigned long long *p, unsigned long long v) { atomicMin(p, v); }
+__device__ __forceinline__ void atomic_max_u64(unsigned long long *p, unsigned long long v) { atomicMax(p, v); }
+__device__ __forceinline__ void atomic_min_u32(unsigned int *p, unsigned int v) { atomicMin(p, v); }
 #endif
 
 // Which entries of a row the column index lists (colidx_kernel's predicate).  row() runs once per row with the whole
@@ -1582,6 +1588,145 @@ __global__ void community_stats_kernel(RowSrc s, const int64_t *__restrict__ row
     if (zn == 0) return;                                     // (warp-uniform)
     for (int i = lane; i < ru.cnt; i += 32)
         if (is_member(ru.vals[i], fu, delta)) atomicAdd(&internal[ru.idx != nullptr ? (int)ru.idx[i] : i], zn);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Cover scores (bigclam_cover_scores): the detected cover X (the communities of is_member, the zero rows in every
+// community or in none) against a truth cover Y given as a CSR of distinct members.  Non-negative doubles order as their
+// bits, so the per-community maxima and minima over t are 64-bit integer atomics and come out the same in any order.
+__device__ __forceinline__ unsigned long long dbl_bits(double d) {
+    return ((unsigned long long)(unsigned)__double2hiint(d) << 32) | (unsigned)__double2loint(d);
+}
+__device__ __forceinline__ double bits_dbl(unsigned long long b) { return __hiloint2double((int)(b >> 32), (int)(unsigned)b); }
+
+// h[m] = -(p log p) with p = m / n, m = 0 .. n (h[0] = 0): the one table every entropy of the cover scores reads.
+__global__ void cover_h_kernel(int64_t n, double *__restrict__ h) {
+    const int64_t m = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (m > n) return;
+    const double p = (double)m / (double)n;
+    h[m] = m == 0 ? 0.0 : -(p * log(p));
+}
+
+// hs[i] = H(S_i) = h(s) + h(n - s) for the sizes s = size[i], i < cnt.
+__global__ void cover_hsize_kernel(const double *__restrict__ h, int64_t n, const int64_t *__restrict__ size, int64_t cnt,
+                                   double *__restrict__ hs) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < cnt) hs[i] = h[size[i]] + h[n - size[i]];
+}
+
+struct CoverArgs {
+    RowSrc s;
+    const double *fmax;                // row_fmax from the count pass; 0: a zero row
+    const int64_t *tptr;               // truth community t = tmem[tptr[t], tptr[t + 1]), distinct ids
+    const int32_t *tmem;
+    const int64_t *xs;                 // |X_c| (the zero rows counted in when zero_rows); 0: an empty community
+    const double *h;                   // cover_h_kernel's table
+    int64_t n;
+    double delta;
+    bool zero_rows;
+    unsigned long long *f1_det;        // per c: bits of max_t F1(c, t), from 0
+    unsigned long long *hc_det;        // per c: bits of min over admissible t of H(X_c | Y_t), from +inf
+    unsigned int *match_det;           // per c (kTies): the smallest t with F1(c, t) == f1_det[c] > 0, from ~0u
+    double *f1_t, *hc_t, *hy_t;        // per t: max_c F1(c, t); min over admissible c of H(Y_t | X_c) (+inf: none); H(Y_t)
+    int32_t *match_t;                  // per t: the smallest c attaining f1_t, -1 when f1_t = 0
+};
+
+// One block per truth community t (empty ones return).  The warps walk t's members u, one member per warp: a zero row
+// adds 1 to z_t, any other row adds 1 to cnt[c] (k counters in shared memory) for each c in M(u), read with row_view +
+// is_member as community_stats_kernel does, so zero rows are never expanded.  Then every non-empty c is a pair (c, t)
+// with a = cnt[c] (+ z_t when zero_rows), x = xs[c], y = |Y_t|:
+//   !kTies  F1 = 2a / (x + y) goes to f1_det[c] (atomicMax on its bits, after a read that skips what cannot improve)
+//           and to the block's maximum (smallest c on ties); an admissible pair's H(X_c | Y_t) goes to hc_det[c]
+//           (atomicMin likewise) and its H(Y_t | X_c) to the block's minimum.  The k x q pairs with a = 0 are evaluated
+//           too: one with x + y > n / 2 can be admissible.
+//   kTies   (after the !kTies launch) every pair whose F1 equals f1_det[c] > 0 offers t to match_det[c] (atomicMin).
+// No floating-point sum depends on the order of the atomics or of the threads.
+constexpr int kCoverWarps = 8;
+template <bool kTies>
+__global__ void __launch_bounds__(32 * kCoverWarps) cover_scores_kernel(CoverArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    __shared__ unsigned int s_zt;
+    __shared__ double s_f1[kCoverWarps], s_hc[kCoverWarps];
+    __shared__ int s_c[kCoverWarps];
+    unsigned int *cnt = reinterpret_cast<unsigned int *>(smem_raw);
+    const int64_t t = blockIdx.x;
+    const int64_t m0 = a.tptr[t], m1 = a.tptr[t + 1];
+    if (m0 == m1) return;                                    // (block-uniform)
+    const int k = a.s.k, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int c = threadIdx.x; c < k; c += blockDim.x) cnt[c] = 0u;
+    if (threadIdx.x == 0) s_zt = 0u;
+    __syncthreads();
+    for (int64_t i = m0 + warp; i < m1; i += kCoverWarps) {
+        const int32_t u = a.tmem[i];
+        const double fu = a.fmax[u];
+        if (fu == 0.0) {                                     // (warp-uniform)
+            if (lane == 0) atomicAdd(&s_zt, 1u);
+            continue;
+        }
+        const RowView r = row_view(a.s, u);
+        for (int j = lane; j < r.cnt; j += 32)
+            if (is_member(r.vals[j], fu, a.delta)) atomicAdd(&cnt[r.idx != nullptr ? (int)r.idx[j] : j], 1u);
+    }
+    __syncthreads();
+    const int64_t n = a.n, y = m1 - m0, zt = a.zero_rows ? (int64_t)s_zt : 0;
+    const double *h = a.h;
+    const double hy = h[y] + h[n - y];
+    double best = 0.0, hmin = INFINITY;
+    int bc = -1;
+    for (int c = threadIdx.x; c < k; c += blockDim.x) {
+        const int64_t x = a.xs[c];
+        if (x == 0) continue;
+        const int64_t ai = (int64_t)cnt[c] + zt;
+        const double f1 = (2.0 * (double)ai) / (double)(x + y);
+        if (kTies) {
+            if (ai > 0 && dbl_bits(f1) == __ldcg(&a.f1_det[c])) atomic_min_u32(&a.match_det[c], (unsigned int)t);
+            continue;
+        }
+        if (f1 > best) {
+            best = f1;
+            bc = c;
+        }
+        if (ai > 0) {
+            const unsigned long long b = dbl_bits(f1);
+            if (b > __ldcg(&a.f1_det[c])) atomic_max_u64(&a.f1_det[c], b);
+        }
+        const double ha = h[ai], hxa = h[x - ai], hya = h[y - ai], hd = h[n - x - y + ai];
+        if (ha + hd > hxa + hya) {                           // admissible (symmetric in X and Y)
+            const double hx = h[x] + h[n - x];
+            const unsigned long long b = dbl_bits(fmax(0.0, ((ha + hxa) + hya) + hd - hy));   // H(X_c | Y_t)
+            if (b < __ldcg(&a.hc_det[c])) atomic_min_u64(&a.hc_det[c], b);
+            hmin = fmin(hmin, fmax(0.0, ((ha + hya) + hxa) + hd - hx));                     // H(Y_t | X_c)
+        }
+    }
+    if (kTies) return;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double ob = __shfl_xor_sync(0xffffffffu, best, o), oh = __shfl_xor_sync(0xffffffffu, hmin, o);
+        const int oc = __shfl_xor_sync(0xffffffffu, bc, o);
+        if (ob > best || (ob == best && (unsigned)oc < (unsigned)bc)) {
+            best = ob;
+            bc = oc;
+        }
+        hmin = fmin(hmin, oh);
+    }
+    if (lane == 0) {
+        s_f1[warp] = best;
+        s_c[warp] = bc;
+        s_hc[warp] = hmin;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    for (int w = 1; w < kCoverWarps; ++w) {
+        if (s_f1[w] > best || (s_f1[w] == best && (unsigned)s_c[w] < (unsigned)bc)) {
+            best = s_f1[w];
+            bc = s_c[w];
+        }
+        hmin = fmin(hmin, s_hc[w]);
+    }
+    a.f1_t[t] = best;
+    a.match_t[t] = best > 0.0 ? bc : -1;
+    a.hc_t[t] = hmin;
+    a.hy_t[t] = hy;
 }
 
 struct SampleArgs {

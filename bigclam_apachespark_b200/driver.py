@@ -496,6 +496,37 @@ class BigClam:
             check(lib.bigclam_community_stats(self._need(), *args), self._ctx)
         return dict(size=size, volume=volume, internal=internal, conductance=cond)
 
+    def score_against(self, truth, delta, zero_rows_everywhere=True):
+        """The communities of extract_communities(delta) scored against a known cover, on the GPU (bigclam_cover_scores,
+        whose header comment defines every output).  truth: a list of int arrays of node ids, the form
+        communities.load_ground_truth() and communities.group() return (any order; a repeated id counts once).
+        zero_rows_everywhere: all-zero rows are in every detected community (as coded) or in none.  Returns dict(avg_f1,
+        nmi_lfk, nmi_max, f1_detected, match_detected, f1_truth, match_truth, hcond_detected, hcond_truth): the scores
+        as floats; per detected community c (length K) and per truth community t (length len(truth)) the best F1, the
+        smallest id attaining it (-1: none) and H*(X_c | Y) / H*(Y_t | X) (NaN outside the NMI)."""
+        lib = _lib.load()
+        K, q = self.K, len(truth)
+        ptr = np.zeros(q + 1, dtype=np.int64)
+        np.cumsum([len(t) for t in truth], out=ptr[1:])
+        members = np.concatenate(truth).astype(np.int64) if q else np.zeros(0, dtype=np.int64)
+        members[(members < 0) | (members > np.iinfo(np.int32).max)] = -1     # rejected by the call, naming the community
+        members = np.ascontiguousarray(members, dtype=np.int32)
+        f1_det, hc_det = np.zeros(K), np.zeros(K)
+        match_det = np.zeros(K, dtype=np.int32)
+        f1_truth, hc_truth = np.zeros(max(q, 1)), np.zeros(max(q, 1))
+        match_truth = np.zeros(max(q, 1), dtype=np.int32)
+        scores = np.zeros(3)
+        args = (float(delta), 1 if zero_rows_everywhere else 0, q, ptr.ctypes.data, members.ctypes.data if len(members) else None,
+                f1_det.ctypes.data, match_det.ctypes.data, f1_truth.ctypes.data, match_truth.ctypes.data, hc_det.ctypes.data,
+                hc_truth.ctypes.data, scores.ctypes.data)
+        if self._multi is not None:
+            self._mcheck(lib.bigclam_multi_cover_scores(self._multi, *args))
+        else:
+            check(lib.bigclam_cover_scores(self._need(), *args), self._ctx)
+        return dict(avg_f1=float(scores[0]), nmi_lfk=float(scores[1]), nmi_max=float(scores[2]), f1_detected=f1_det,
+                    match_detected=match_det, f1_truth=f1_truth[:q], match_truth=match_truth[:q], hcond_detected=hc_det,
+                    hcond_truth=hc_truth[:q])
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

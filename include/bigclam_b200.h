@@ -343,6 +343,53 @@ int bigclam_multi_community_stats(bigclam_multi *m, double delta, int32_t zero_r
                                   int64_t *internal_out, double *conductance_out);
 
 /*
+ * The communities of the current F scored against a known cover: Avg-F1 and overlapping NMI.
+ *
+ * Detected cover X: the communities of bigclam_extract_grouped at delta (the rule above), the all-zero rows in every
+ * community (zero_rows = 1, as coded) or in none (0); X_c is community c, and only non-empty ones take part.  It is
+ * the cover communities.group(..., zero_rows_everywhere) returns.  Truth cover Y: q communities as a CSR, truth_ptr
+ * (q + 1, int64, truth_ptr[0] = 0, non-decreasing) and truth_members (int32 ids in [0, n)); members may come in any
+ * order and a repeated id counts once.  Y may be a ground truth or the group() output of another fit.
+ *
+ * For a non-empty X_c and a non-empty Y_t, with x = |X_c|, y = |Y_t|, a = |X_c ∩ Y_t| and n the context's node count:
+ *   F1(c, t) = (2.0 * a) / (double)(x + y)                  (the integer sum exact; communities.avg_f1's expression)
+ *   f1_det[c]    = max over t of F1(c, t);  match_det[c] = the smallest t attaining it.  An empty c, or a best F1 of 0,
+ *                  gives 0 and -1.  f1_truth[t] / match_truth[t]: the same in the other direction; an empty Y_t gives
+ *                  0 and -1 and still counts in the mean.
+ *   scores_out[0] avg_f1 = 0.5 * (mean of f1_det over the non-empty c + mean of f1_truth over all q); 0 when there is
+ *                  no non-empty c or q = 0 (as communities.avg_f1).
+ * Overlapping NMI (Lancichinetti, Fortunato & Kertész 2009), natural logarithms, h of an integer count m:
+ *   h(m)          = m == 0 ? 0 : -(p * log(p)),  p = (double)m / (double)n
+ *   H(X_c)        = h(x) + h(n - x)
+ *   H(X_c | Y_t)  = max(0, ((h(a) + h(x - a)) + h(y - a)) + h(n - x - y + a) - (h(y) + h(n - y)))
+ *   (c, t) is admissible iff h(a) + h(n - x - y + a) > h(x - a) + h(y - a)   (symmetric in X and Y)
+ *   hcond_det[c]  = H*(X_c | Y) = the minimum of H(X_c | Y_t) over the admissible t, or H(X_c) when none is;
+ *                   hcond_truth[t] = H*(Y_t | X) the same in the other direction (x and y, X and Y swapped).
+ *                   Only communities with 0 < size < n enter the NMI; the others get NaN.
+ *   scores_out[1] nmi_lfk = 1 - 0.5 * (mean_c H*(X_c|Y) / H(X_c) + mean_t H*(Y_t|X) / H(Y_t))
+ *   scores_out[2] nmi_max = 0.5 * ((ΣH(X_c) - ΣH*(X_c|Y)) + (ΣH(Y_t) - ΣH*(Y_t|X))) / max(ΣH(X_c), ΣH(Y_t))
+ *                 (McDaid, Greene & Hurley 2011).  Either NMI is NaN when one side has no community of size in (0, n).
+ * Every mean and sum is a left fold in ascending id.  Scoring a fit against its own group() output in the same mode
+ * gives exactly 1.0 for all three scores (the max(0, .) makes the self pair exactly 0).
+ *
+ * f1_det, match_det (k each), f1_truth, match_truth (q each, may be NULL when q = 0) and scores_out (3) are required;
+ * hcond_det (k) and hcond_truth (q) are optional.  BIGCLAM_EINVAL before any device work for delta <= 0 or NaN (+inf
+ * allowed), zero_rows not 0 or 1, q < 0 or q >= 2^31, truth_ptr[0] != 0, a decreasing truth_ptr, an id outside [0, n)
+ * (naming the truth community) or a NULL required argument; a negative entry of F gives BIGCLAM_EUNSUPPORTED naming the
+ * smallest such row.  The outputs depend on (F bits, delta, zero_rows, the truth sets) only: not on the row layout, the
+ * order of truth members or repeats, the number of GPUs or the device.  Device scratch is O(n + k + q + Σ|Y_t|), nothing
+ * n x k (BIGCLAM_ENOMEM when even that cannot be allocated).  Reads F only (no state changes), on the context's stream,
+ * synchronous.  The multi-GPU call reads rank 0's replica; its errors go to bigclam_multi_last_error.
+ */
+int bigclam_cover_scores(bigclam_ctx *ctx, double delta, int32_t zero_rows, int64_t q, const int64_t *truth_ptr /* q + 1 */,
+                         const int32_t *truth_members /* truth_ptr[q] */, double *f1_det /* k */, int32_t *match_det /* k */,
+                         double *f1_truth /* q */, int32_t *match_truth /* q */, double *hcond_det /* k, optional */,
+                         double *hcond_truth /* q, optional */, double *scores_out /* 3: avg_f1, nmi_lfk, nmi_max */);
+int bigclam_multi_cover_scores(bigclam_multi *m, double delta, int32_t zero_rows, int64_t q, const int64_t *truth_ptr,
+                               const int32_t *truth_members, double *f1_det, int32_t *match_det, double *f1_truth,
+                               int32_t *match_truth, double *hcond_det, double *hcond_truth, double *scores_out);
+
+/*
  * The fitted model as a model of edges (the clamp of bigclam4-7.scala:166, the edge term of :218), on the current F:
  *   x_uv = sum of F_uc * F_vc over the components c that are non-zero in both rows, folded left in ascending c with
  *          every product and every sum rounded on its own (the same bits for sparse and dense rows and for (v, u));

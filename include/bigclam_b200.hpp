@@ -18,6 +18,7 @@
 //   community extraction         Bigclamv2.scala:223-230         delta_threshold(), extract(delta),
 //                                                                extract_grouped(delta, ...)
 //   community scores, the formula of conductanceLocalMin :64-67  community_stats(delta, zero_rows_everywhere)
+//   Avg-F1 (thesis p.21) and overlapping NMI against a known cover  score_against(truth, delta, zero_rows_everywhere)
 //   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m),
 //                                                                sample_graph(seed, eps)
 //   rows for new nodes, the fit held fixed (:157-184 per node)    fold_in(rowptr, col, max_iter, rel_tol, ...)
@@ -261,6 +262,48 @@ public:
         check(multi_ ? bigclam_multi_community_stats(multi_, delta, zr, s.size.data(), s.volume.data(), s.internal.data(), s.conductance.data())
                      : bigclam_community_stats(ctx_, delta, zr, s.size.data(), s.volume.data(), s.internal.data(), s.conductance.data()),
               "community_stats");
+        return s;
+    }
+
+    // The communities of extract(delta) scored against a known cover (bigclam_cover_scores, whose header comment defines
+    // every output): truth is a list of node-id lists (any order; a repeated id counts once).  Avg-F1 and the two
+    // overlapping NMIs, and per community of either side its best F1, the smallest id attaining it (-1: none) and
+    // H*(X_c | Y) / H*(Y_t | X) (NaN outside the NMI).  zero_rows_everywhere: all-zero rows in every detected community
+    // (as coded) or in none.  Works for multi-GPU handles too.
+    struct CoverScores {
+        double avg_f1 = 0.0, nmi_lfk = 0.0, nmi_max = 0.0;
+        std::vector<double> f1_detected, f1_truth, hcond_detected, hcond_truth;
+        std::vector<int32_t> match_detected, match_truth;
+    };
+    CoverScores score_against(const std::vector<std::vector<int32_t>> &truth, double delta, bool zero_rows_everywhere = true) {
+        need();
+        const size_t q = truth.size();
+        std::vector<int64_t> ptr(q + 1, 0);
+        for (size_t t = 0; t < q; ++t) ptr[t + 1] = ptr[t] + (int64_t)truth[t].size();
+        std::vector<int32_t> members;
+        members.reserve((size_t)ptr[q]);
+        for (const auto &y : truth) members.insert(members.end(), y.begin(), y.end());
+        CoverScores s;
+        s.f1_detected.assign((size_t)K_, 0.0);
+        s.hcond_detected.assign((size_t)K_, 0.0);
+        s.match_detected.assign((size_t)K_, -1);
+        s.f1_truth.assign(std::max<size_t>(q, 1), 0.0);
+        s.hcond_truth.assign(std::max<size_t>(q, 1), 0.0);
+        s.match_truth.assign(std::max<size_t>(q, 1), -1);
+        double scores[3] = {0.0, 0.0, 0.0};
+        const int32_t zr = zero_rows_everywhere ? 1 : 0;
+        const int32_t *mp = members.empty() ? nullptr : members.data();
+        check(multi_ ? bigclam_multi_cover_scores(multi_, delta, zr, (int64_t)q, ptr.data(), mp, s.f1_detected.data(), s.match_detected.data(),
+                                                  s.f1_truth.data(), s.match_truth.data(), s.hcond_detected.data(), s.hcond_truth.data(), scores)
+                     : bigclam_cover_scores(ctx_, delta, zr, (int64_t)q, ptr.data(), mp, s.f1_detected.data(), s.match_detected.data(),
+                                            s.f1_truth.data(), s.match_truth.data(), s.hcond_detected.data(), s.hcond_truth.data(), scores),
+              "score_against");
+        s.f1_truth.resize(q);
+        s.hcond_truth.resize(q);
+        s.match_truth.resize(q);
+        s.avg_f1 = scores[0];
+        s.nmi_lfk = scores[1];
+        s.nmi_max = scores[2];
         return s;
     }
 
