@@ -78,7 +78,8 @@ int bigclam_step_sizes(double beta, int32_t max_inter, double *out);
 /*
  * Context = the hot path's resident state: CSR adjacency (collectNeighbor, :50-51), F double
  * buffer, sumF.  rowptr has n+1 entries, col has rowptr[n] entries in [0,n); neighbour lists are
- * taken as given (multiplicity and order preserved, like collectNeighborIds(Either)).
+ * taken as given (multiplicity and order preserved, like collectNeighborIds(Either)): repeated entries,
+ * self loops, unsorted and one-sided lists are tested on every step engine in tests/test_gpu_graphx_lists.py.
  * Replaces: Neightborbc broadcast (:51) and the per-call Fbc broadcast (:154).
  * Limits on k: 1024 for dense rows, 16384 with BIGCLAM_F_SPARSE_ROWS; above them BIGCLAM_EUNSUPPORTED (checked
  * before any device is touched).
