@@ -2713,6 +2713,23 @@ static int mfail(bigclam_multi *m, int code, const char *fmt, ...) {
 }
 static int mfail_from(bigclam_multi *m, int code, bigclam_ctx *c) { return mfail(m, code, "%s", bigclam_last_error(c)); }
 
+// The forwarders below run f on one rank, or on every rank in rank order up to the first error, and report the failing
+// rank's message.  The read-only queries run on rank 0: all replicas hold the same rows.
+template <typename... P, typename... A>
+static int on_rank(bigclam_multi *m, int32_t rank, int (*f)(bigclam_ctx *, P...), A... args) {
+    if (m == nullptr || rank < 0 || rank >= m->world) return BIGCLAM_EINVAL;
+    bigclam_ctx *c = m->r[(size_t)rank];
+    const int rc = f(c, args...);
+    return rc != BIGCLAM_OK ? mfail_from(m, rc, c) : BIGCLAM_OK;
+}
+template <typename... P, typename... A>
+static int on_every_rank(bigclam_multi *m, int (*f)(bigclam_ctx *, P...), A... args) {
+    if (m == nullptr) return BIGCLAM_EINVAL;
+    for (bigclam_ctx *c : m->r)
+        if (const int rc = f(c, args...); rc != BIGCLAM_OK) return mfail_from(m, rc, c);
+    return BIGCLAM_OK;
+}
+
 extern "C" const char *bigclam_multi_last_error(const bigclam_multi *m) { return m != nullptr ? m->err.c_str() : g_multi_err.c_str(); }
 
 extern "C" void bigclam_multi_destroy(bigclam_multi *m) {
@@ -2817,113 +2834,56 @@ extern "C" int bigclam_multi_create(bigclam_multi **out, int64_t n, const int64_
     return BIGCLAM_OK;
 }
 
-#define MCALL(expr, c)                                           \
-    do {                                                         \
-        int rc__ = (expr);                                       \
-        if (rc__ != BIGCLAM_OK) return mfail_from(m, rc__, c);   \
-    } while (0)
-
-extern "C" int bigclam_multi_set_F(bigclam_multi *m, const double *F) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    for (bigclam_ctx *c : m->r) MCALL(bigclam_set_F(c, F), c);
-    return BIGCLAM_OK;
-}
+extern "C" int bigclam_multi_set_F(bigclam_multi *m, const double *F) { return on_every_rank(m, bigclam_set_F, F); }
 extern "C" int bigclam_multi_set_F_csr(bigclam_multi *m, const int64_t *indptr, const int32_t *indices, const double *values) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    for (bigclam_ctx *c : m->r) MCALL(bigclam_set_F_csr(c, indptr, indices, values), c);
-    return BIGCLAM_OK;
+    return on_every_rank(m, bigclam_set_F_csr, indptr, indices, values);
 }
 extern "C" int bigclam_multi_init_F(bigclam_multi *m, const int32_t *ranked_seeds, int64_t n_ranked, int32_t include_self, uint64_t pad_seed) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    for (bigclam_ctx *c : m->r) MCALL(bigclam_init_F(c, ranked_seeds, n_ranked, include_self, pad_seed), c);
-    return BIGCLAM_OK;
+    return on_every_rank(m, bigclam_init_F, ranked_seeds, n_ranked, include_self, pad_seed);
 }
-extern "C" int bigclam_multi_set_sumF(bigclam_multi *m, const double *sumF) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    for (bigclam_ctx *c : m->r) MCALL(bigclam_set_sumF(c, sumF), c);
-    return BIGCLAM_OK;
-}
-extern "C" int bigclam_multi_get_F(bigclam_multi *m, int32_t rank, double *F_out) {
-    if (m == nullptr || rank < 0 || rank >= m->world) return BIGCLAM_EINVAL;
-    MCALL(bigclam_get_F(m->r[(size_t)rank], F_out), m->r[(size_t)rank]);
-    return BIGCLAM_OK;
-}
-extern "C" int bigclam_multi_get_sumF(bigclam_multi *m, int32_t rank, double *sumF_out) {
-    if (m == nullptr || rank < 0 || rank >= m->world) return BIGCLAM_EINVAL;
-    MCALL(bigclam_get_sumF(m->r[(size_t)rank], sumF_out), m->r[(size_t)rank]);
-    return BIGCLAM_OK;
-}
-extern "C" int bigclam_multi_get_F_nnz(bigclam_multi *m, int64_t *nnz_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_get_F_nnz(m->r[0], nnz_out), m->r[0]);
-    return BIGCLAM_OK;
-}
+extern "C" int bigclam_multi_set_sumF(bigclam_multi *m, const double *sumF) { return on_every_rank(m, bigclam_set_sumF, sumF); }
+extern "C" int bigclam_multi_get_F(bigclam_multi *m, int32_t rank, double *F_out) { return on_rank(m, rank, bigclam_get_F, F_out); }
+extern "C" int bigclam_multi_get_sumF(bigclam_multi *m, int32_t rank, double *sumF_out) { return on_rank(m, rank, bigclam_get_sumF, sumF_out); }
+extern "C" int bigclam_multi_get_F_nnz(bigclam_multi *m, int64_t *nnz_out) { return on_rank(m, 0, bigclam_get_F_nnz, nnz_out); }
 extern "C" int bigclam_multi_get_F_csr(bigclam_multi *m, int64_t *indptr_out, int32_t *indices_out, double *values_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_get_F_csr(m->r[0], indptr_out, indices_out, values_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_get_F_csr, indptr_out, indices_out, values_out);
 }
-
-// Edge probabilities and recommendations read rank 0's replica (all replicas hold the same rows).
 extern "C" int bigclam_multi_pair_affinity(bigclam_multi *m, const int32_t *u, const int32_t *v, int64_t count, double *x_out, double *p_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_pair_affinity(m->r[0], u, v, count, x_out, p_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_pair_affinity, u, v, count, x_out, p_out);
 }
 extern "C" int bigclam_multi_recommend(bigclam_multi *m, const int32_t *nodes, int64_t count, int32_t mm, int32_t *v_out, double *x_out,
                                        int32_t *found_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_recommend(m->r[0], nodes, count, mm, v_out, x_out, found_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_recommend, nodes, count, mm, v_out, x_out, found_out);
 }
 extern "C" int bigclam_multi_sample_graph_nnz(bigclam_multi *m, uint64_t seed, double eps, int64_t *nnz_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_sample_graph_nnz(m->r[0], seed, eps, nnz_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_sample_graph_nnz, seed, eps, nnz_out);
 }
 extern "C" int bigclam_multi_sample_graph(bigclam_multi *m, uint64_t seed, double eps, int64_t *rowptr_out, int32_t *col_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_sample_graph(m->r[0], seed, eps, rowptr_out, col_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_sample_graph, seed, eps, rowptr_out, col_out);
 }
 extern "C" int bigclam_multi_fold_in_nnz(bigclam_multi *m, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter,
                                          double rel_tol, int64_t *nnz_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_fold_in_nnz(m->r[0], q, rowptr, col, max_iter, rel_tol, nnz_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_fold_in_nnz, q, rowptr, col, max_iter, rel_tol, nnz_out);
 }
 extern "C" int bigclam_multi_fold_in(bigclam_multi *m, int64_t q, const int64_t *rowptr, const int32_t *col, int32_t max_iter, double rel_tol,
                                      int64_t *indptr_out, int32_t *indices_out, double *values_out, double *llh_out, int32_t *iters_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_fold_in(m->r[0], q, rowptr, col, max_iter, rel_tol, indptr_out, indices_out, values_out, llh_out, iters_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_fold_in, q, rowptr, col, max_iter, rel_tol, indptr_out, indices_out, values_out, llh_out, iters_out);
 }
 extern "C" int bigclam_multi_extract_nnz(bigclam_multi *m, double delta, int64_t *nnz_out, int64_t *n_zero_rows_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_extract_nnz(m->r[0], delta, nnz_out, n_zero_rows_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_extract_nnz, delta, nnz_out, n_zero_rows_out);
 }
 extern "C" int bigclam_multi_extract_grouped(bigclam_multi *m, double delta, int64_t *comptr_out, int32_t *members_out, int32_t *zero_rows_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_extract_grouped(m->r[0], delta, comptr_out, members_out, zero_rows_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_extract_grouped, delta, comptr_out, members_out, zero_rows_out);
 }
-
 extern "C" int bigclam_multi_community_stats(bigclam_multi *m, double delta, int32_t zero_rows, int64_t *size_out, int64_t *volume_out,
                                              int64_t *internal_out, double *conductance_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_community_stats(m->r[0], delta, zero_rows, size_out, volume_out, internal_out, conductance_out), m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_community_stats, delta, zero_rows, size_out, volume_out, internal_out, conductance_out);
 }
-
 extern "C" int bigclam_multi_cover_scores(bigclam_multi *m, double delta, int32_t zero_rows, int64_t q, const int64_t *truth_ptr,
                                           const int32_t *truth_members, double *f1_det, int32_t *match_det, double *f1_truth,
                                           int32_t *match_truth, double *hcond_det, double *hcond_truth, double *scores_out) {
-    if (m == nullptr) return BIGCLAM_EINVAL;
-    MCALL(bigclam_cover_scores(m->r[0], delta, zero_rows, q, truth_ptr, truth_members, f1_det, match_det, f1_truth, match_truth,
-                               hcond_det, hcond_truth, scores_out),
-          m->r[0]);
-    return BIGCLAM_OK;
+    return on_rank(m, 0, bigclam_cover_scores, delta, zero_rows, q, truth_ptr, truth_members, f1_det, match_det, f1_truth, match_truth,
+                   hcond_det, hcond_truth, scores_out);
 }
 
 extern "C" int bigclam_multi_loglikelihood(bigclam_multi *m, double *llh_out) {
@@ -2977,4 +2937,3 @@ extern "C" int bigclam_multi_get_ls_stats(bigclam_multi *m, int64_t *nodes_asked
 }
 
 extern "C" int bigclam_multi_world(const bigclam_multi *m) { return m != nullptr ? m->world : BIGCLAM_EINVAL; }
-#undef MCALL

@@ -152,6 +152,20 @@ class BigClam:
         if rc != _lib.OK:
             raise _lib.BigclamError(rc, (_lib.load().bigclam_multi_last_error(self._multi) or b"").decode())
 
+    def _call(self, name, *args):
+        """bigclam_multi_<name>(multi handle, *args) on a multi handle, else bigclam_<name>(context, *args)."""
+        lib = _lib.load()
+        if self._multi is not None:
+            self._mcheck(getattr(lib, "bigclam_multi_" + name)(self._multi, *args))
+        else:
+            check(getattr(lib, "bigclam_" + name)(self._need(), *args), self._ctx)
+
+    def _set_sumF(self, sumF):
+        if sumF is not None:
+            sumF = np.ascontiguousarray(sumF, dtype=np.float64)
+            self._call("set_sumF", sumF.ctypes.data)
+        return self
+
     def set_F_csr(self, indptr, indices, values, K=None, sumF=None):
         """F <- CSR rows (the reference's RDD[(Long, BSV[Double])], :97-104); sumF <- column sums unless given.
         With sparse_rows=True no dense n x K image is built anywhere."""
@@ -162,33 +176,17 @@ class BigClam:
             self.set_K(int(K))
         if len(indptr) != self.n + 1 or len(indices) != indptr[-1] or len(values) != indptr[-1]:
             raise ValueError("CSR arrays do not describe n rows")
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_set_F_csr(self._multi, indptr.ctypes.data, indices.ctypes.data, values.ctypes.data))
-            if sumF is not None:
-                sumF = np.ascontiguousarray(sumF, dtype=np.float64)
-                self._mcheck(_lib.load().bigclam_multi_set_sumF(self._multi, sumF.ctypes.data))
-            return self
-        check(_lib.load().bigclam_set_F_csr(self._need(), indptr.ctypes.data, indices.ctypes.data, values.ctypes.data), self._ctx)
-        if sumF is not None:
-            sumF = np.ascontiguousarray(sumF, dtype=np.float64)
-            check(_lib.load().bigclam_set_sumF(self._ctx, sumF.ctypes.data), self._ctx)
-        return self
+        self._call("set_F_csr", indptr.ctypes.data, indices.ctypes.data, values.ctypes.data)
+        return self._set_sumF(sumF)
 
     def F_csr(self):
         """Current F as (indptr, indices, values): ascending indices inside a row, no stored zeros."""
-        lib = _lib.load()
         nnz = C.c_int64()
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_get_F_nnz(self._multi, C.byref(nnz)))
-        else:
-            check(lib.bigclam_get_F_nnz(self._need(), C.byref(nnz)), self._ctx)
+        self._call("get_F_nnz", C.byref(nnz))
         indptr = np.empty(self.n + 1, dtype=np.int64)
         indices = np.empty(max(nnz.value, 1), dtype=np.int32)
         values = np.empty(max(nnz.value, 1), dtype=np.float64)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_get_F_csr(self._multi, indptr.ctypes.data, indices.ctypes.data, values.ctypes.data))
-        else:
-            check(lib.bigclam_get_F_csr(self._ctx, indptr.ctypes.data, indices.ctypes.data, values.ctypes.data), self._ctx)
+        self._call("get_F_csr", indptr.ctypes.data, indices.ctypes.data, values.ctypes.data)
         return indptr, indices[:nnz.value], values[:nnz.value]
 
     def set_F(self, F, sumF=None):
@@ -201,17 +199,8 @@ class BigClam:
             self.set_K(F.shape[1])
         if F.shape != (self.n, self.K):
             raise ValueError(f"F must be {self.n} x {self.K}")
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_set_F(self._multi, F.ctypes.data))
-            if sumF is not None:
-                sumF = np.ascontiguousarray(sumF, dtype=np.float64)
-                self._mcheck(_lib.load().bigclam_multi_set_sumF(self._multi, sumF.ctypes.data))
-            return self
-        check(_lib.load().bigclam_set_F(self._ctx, F.ctypes.data), self._ctx)
-        if sumF is not None:
-            sumF = np.ascontiguousarray(sumF, dtype=np.float64)
-            check(_lib.load().bigclam_set_sumF(self._ctx, sumF.ctypes.data), self._ctx)
-        return self
+        self._call("set_F", F.ctypes.data)
+        return self._set_sumF(sumF)
 
     def replica_F(self, rank: int = 0) -> np.ndarray:
         """numGPUs > 1: the F replica of one rank (all replicas are identical after every call)."""
@@ -271,11 +260,7 @@ class BigClam:
         if (self._ctx is None and self._multi is None) or int(K) != self.K:
             self.set_K(int(K))
         seeds = np.ascontiguousarray(self.Sbc, dtype=np.int32)
-        args = (seeds.ctypes.data, len(seeds), 1 if include_self else 0, C.c_uint64(pad_seed))
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_init_F(self._multi, *args))
-        else:
-            check(_lib.load().bigclam_init_F(self._ctx, *args), self._ctx)
+        self._call("init_F", seeds.ctypes.data, len(seeds), 1 if include_self else 0, C.c_uint64(pad_seed))
         return self
 
     def initNeighborComF(self, K: int, include_self: bool = False, pad_seed: int = 1234):
@@ -293,32 +278,21 @@ class BigClam:
             mask_ptr = mask.ctypes.data
         llh = C.c_double()
         nupd = C.c_int64()
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_step(self._multi, mask_ptr, C.byref(llh), C.byref(nupd)))
-        else:
-            check(_lib.load().bigclam_step(self._need(), mask_ptr, C.byref(llh), C.byref(nupd)), self._ctx)
+        self._call("step", mask_ptr, C.byref(llh), C.byref(nupd))
         self.last_n_updated = nupd.value
         return llh.value
 
     def loglikelihood(self) -> float:
         """bigclamv3-7.scala:106-120 / Bigclamv2.scala:187-200."""
         llh = C.c_double()
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_loglikelihood(self._multi, C.byref(llh)))
-        else:
-            check(_lib.load().bigclam_loglikelihood(self._need(), C.byref(llh)), self._ctx)
+        self._call("loglikelihood", C.byref(llh))
         return llh.value
 
     def _run(self, variant: int, rel_tol: float, max_outer: int, trace_cap: int = 65536):
         trace = np.full(trace_cap, np.nan)
         llh = C.c_double()
         calls = C.c_int64()
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_run(self._multi, variant, rel_tol, max_outer, C.byref(llh), C.byref(calls),
-                                                       trace.ctypes.data, trace_cap))
-        else:
-            check(_lib.load().bigclam_run(self._need(), variant, rel_tol, max_outer, C.byref(llh), C.byref(calls),
-                                          trace.ctypes.data, trace_cap), self._ctx)
+        self._call("run", variant, rel_tol, max_outer, C.byref(llh), C.byref(calls), trace.ctypes.data, trace_cap)
         self.last_calls = calls.value
         self.last_trace = trace[:min(calls.value, trace_cap)]
         return llh.value
@@ -376,12 +350,7 @@ class BigClam:
             raise ValueError("u and v must have the same length")
         x = np.empty(len(u), dtype=np.float64)
         p = np.empty(len(u), dtype=np.float64)
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_pair_affinity(self._multi, u.ctypes.data, v.ctypes.data, len(u),
-                                                                 x.ctypes.data, p.ctypes.data))
-        else:
-            check(_lib.load().bigclam_pair_affinity(self._need(), u.ctypes.data, v.ctypes.data, len(u), x.ctypes.data,
-                                                    p.ctypes.data), self._ctx)
+        self._call("pair_affinity", u.ctypes.data, v.ctypes.data, len(u), x.ctypes.data, p.ctypes.data)
         return x, p
 
     def recommend(self, nodes=None, m: int = 10):
@@ -395,10 +364,7 @@ class BigClam:
         m = int(m)
         vo = np.empty((cnt, max(m, 0)), dtype=np.int32)
         xo = np.empty((cnt, max(m, 0)), dtype=np.float64)
-        if self._multi is not None:
-            self._mcheck(_lib.load().bigclam_multi_recommend(self._multi, ptr, cnt, m, vo.ctypes.data, xo.ctypes.data, None))
-        else:
-            check(_lib.load().bigclam_recommend(self._need(), ptr, cnt, m, vo.ctypes.data, xo.ctypes.data, None), self._ctx)
+        self._call("recommend", ptr, cnt, m, vo.ctypes.data, xo.ctypes.data, None)
         return vo, xo
 
     def sample_graph(self, seed, eps=0.0):
@@ -406,19 +372,12 @@ class BigClam:
         p of edge_probability), any other pair with probability eps (0 <= eps < 1; 1 - MAX_P_ is the model as coded).
         The same (F, seed, eps) gives the same graph.  Returns (rowptr int64[n + 1], col int32[nnz]): symmetric, rows
         ascending, no self loops, the shape set_graph takes."""
-        lib = _lib.load()
         seed, eps = int(seed) & 0xFFFFFFFFFFFFFFFF, float(eps)
         nnz = C.c_int64()
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_sample_graph_nnz(self._multi, seed, eps, C.byref(nnz)))
-        else:
-            check(lib.bigclam_sample_graph_nnz(self._need(), seed, eps, C.byref(nnz)), self._ctx)
+        self._call("sample_graph_nnz", seed, eps, C.byref(nnz))
         rowptr = np.empty(self.n + 1, dtype=np.int64)
         col = np.empty(max(nnz.value, 1), dtype=np.int32)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_sample_graph(self._multi, seed, eps, rowptr.ctypes.data, col.ctypes.data))
-        else:
-            check(lib.bigclam_sample_graph(self._ctx, seed, eps, rowptr.ctypes.data, col.ctypes.data), self._ctx)
+        self._call("sample_graph", seed, eps, rowptr.ctypes.data, col.ctypes.data)
         return rowptr, col[:nnz.value]
 
     def fold_in(self, rowptr, col, max_iter: int = 100, rel_tol: float = 1e-4):
@@ -427,7 +386,6 @@ class BigClam:
         reference's line searches on its own objective, stopping when none passes or the LLH gains less than rel_tol
         (relative).  Nodes never see each other.  Returns (indptr int64[q + 1], indices int32[nnz], values float64[nnz],
         llh float64[q], iters int32[q]): rows ascending without zeros, the shape set_F_csr takes."""
-        lib = _lib.load()
         rowptr = np.ascontiguousarray(rowptr, dtype=np.int64).ravel()
         col = np.ascontiguousarray(col, dtype=np.int32).ravel()
         if len(rowptr) < 1:
@@ -438,20 +396,13 @@ class BigClam:
         max_iter, rel_tol = int(max_iter), float(rel_tol)
         nnz = C.c_int64()
         args = (q, rowptr.ctypes.data, col.ctypes.data, max_iter, rel_tol)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_fold_in_nnz(self._multi, *args, C.byref(nnz)))
-        else:
-            check(lib.bigclam_fold_in_nnz(self._need(), *args, C.byref(nnz)), self._ctx)
+        self._call("fold_in_nnz", *args, C.byref(nnz))
         indptr = np.zeros(q + 1, dtype=np.int64)
         indices = np.empty(max(nnz.value, 1), dtype=np.int32)
         values = np.empty(max(nnz.value, 1), dtype=np.float64)
         llh = np.zeros(q, dtype=np.float64)
         iters = np.zeros(q, dtype=np.int32)
-        outs = (indptr.ctypes.data, indices.ctypes.data, values.ctypes.data, llh.ctypes.data, iters.ctypes.data)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_fold_in(self._multi, *args, *outs))
-        else:
-            check(lib.bigclam_fold_in(self._ctx, *args, *outs), self._ctx)
+        self._call("fold_in", *args, indptr.ctypes.data, indices.ctypes.data, values.ctypes.data, llh.ctypes.data, iters.ctypes.data)
         return indptr, indices[:nnz.value], values[:nnz.value], llh, iters
 
     def extract_communities(self, delta):
@@ -460,21 +411,13 @@ class BigClam:
         int32[z]): community c is members[comptr[c]:comptr[c + 1]] ascending; an all-zero row is, as coded, a member of
         every community and is listed once in zero_rows (ascending) instead.  communities.group() turns this into
         communities.extract()'s lists."""
-        lib = _lib.load()
         delta = float(delta)
         nnz, z = C.c_int64(), C.c_int64()
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_extract_nnz(self._multi, delta, C.byref(nnz), C.byref(z)))
-        else:
-            check(lib.bigclam_extract_nnz(self._need(), delta, C.byref(nnz), C.byref(z)), self._ctx)
+        self._call("extract_nnz", delta, C.byref(nnz), C.byref(z))
         comptr = np.zeros(self.K + 1, dtype=np.int64)
         members = np.empty(max(nnz.value, 1), dtype=np.int32)
         zero_rows = np.empty(max(z.value, 1), dtype=np.int32)
-        outs = (comptr.ctypes.data, members.ctypes.data, zero_rows.ctypes.data)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_extract_grouped(self._multi, delta, *outs))
-        else:
-            check(lib.bigclam_extract_grouped(self._ctx, delta, *outs), self._ctx)
+        self._call("extract_grouped", delta, comptr.ctypes.data, members.ctypes.data, zero_rows.ctypes.data)
         return comptr, members[:nnz.value], zero_rows[:z.value]
 
     def community_stats(self, delta, zero_rows_everywhere=True):
@@ -484,16 +427,11 @@ class BigClam:
         formula (bigclam4-7.scala:64-67) with cut = volume - internal, vol_S = internal and sigma = the number of list
         entries of the graph (an empty community scores 0).  zero_rows_everywhere: all-zero rows are in every community
         (as coded) or in none, the two choices of communities.group()."""
-        lib = _lib.load()
         K = self.K
         size, volume, internal = (np.zeros(K, dtype=np.int64) for _ in range(3))
         cond = np.zeros(K, dtype=np.float64)
-        args = (float(delta), 1 if zero_rows_everywhere else 0, size.ctypes.data, volume.ctypes.data, internal.ctypes.data,
-                cond.ctypes.data)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_community_stats(self._multi, *args))
-        else:
-            check(lib.bigclam_community_stats(self._need(), *args), self._ctx)
+        self._call("community_stats", float(delta), 1 if zero_rows_everywhere else 0, size.ctypes.data, volume.ctypes.data,
+                   internal.ctypes.data, cond.ctypes.data)
         return dict(size=size, volume=volume, internal=internal, conductance=cond)
 
     def score_against(self, truth, delta, zero_rows_everywhere=True):
@@ -504,7 +442,6 @@ class BigClam:
         nmi_lfk, nmi_max, f1_detected, match_detected, f1_truth, match_truth, hcond_detected, hcond_truth): the scores
         as floats; per detected community c (length K) and per truth community t (length len(truth)) the best F1, the
         smallest id attaining it (-1: none) and H*(X_c | Y) / H*(Y_t | X) (NaN outside the NMI)."""
-        lib = _lib.load()
         K, q = self.K, len(truth)
         ptr = np.zeros(q + 1, dtype=np.int64)
         np.cumsum([len(t) for t in truth], out=ptr[1:])
@@ -516,13 +453,9 @@ class BigClam:
         f1_truth, hc_truth = np.zeros(max(q, 1)), np.zeros(max(q, 1))
         match_truth = np.zeros(max(q, 1), dtype=np.int32)
         scores = np.zeros(3)
-        args = (float(delta), 1 if zero_rows_everywhere else 0, q, ptr.ctypes.data, members.ctypes.data if len(members) else None,
-                f1_det.ctypes.data, match_det.ctypes.data, f1_truth.ctypes.data, match_truth.ctypes.data, hc_det.ctypes.data,
-                hc_truth.ctypes.data, scores.ctypes.data)
-        if self._multi is not None:
-            self._mcheck(lib.bigclam_multi_cover_scores(self._multi, *args))
-        else:
-            check(lib.bigclam_cover_scores(self._need(), *args), self._ctx)
+        self._call("cover_scores", float(delta), 1 if zero_rows_everywhere else 0, q, ptr.ctypes.data,
+                   members.ctypes.data if len(members) else None, f1_det.ctypes.data, match_det.ctypes.data, f1_truth.ctypes.data,
+                   match_truth.ctypes.data, hc_det.ctypes.data, hc_truth.ctypes.data, scores.ctypes.data)
         return dict(avg_f1=float(scores[0]), nmi_lfk=float(scores[1]), nmi_max=float(scores[2]), f1_detected=f1_det,
                     match_detected=match_det, f1_truth=f1_truth[:q], match_truth=match_truth[:q], hcond_detected=hc_det,
                     hcond_truth=hc_truth[:q])
@@ -561,10 +494,7 @@ class BigClam:
         """Sparse rows: dict(nodes_asked, nodes_searched) of the tile path since the previous read — how many of the
         nodes that asked for a line search had a candidate the bounds could not exclude."""
         a, b = C.c_int64(), C.c_int64()
-        if self._multi is not None:          # summed over the ranks (every rank counts the nodes it owns)
-            self._mcheck(_lib.load().bigclam_multi_get_ls_stats(self._multi, C.byref(a), C.byref(b)))
-            return {"nodes_asked": a.value, "nodes_searched": b.value}
-        check(_lib.load().bigclam_get_ls_stats(self._need(), C.byref(a), C.byref(b)), self._ctx)
+        self._call("get_ls_stats", C.byref(a), C.byref(b))          # multi handle: summed over the ranks
         return {"nodes_asked": a.value, "nodes_searched": b.value}
 
     def set_stream(self, cuda_stream: int):

@@ -135,8 +135,8 @@ public:
     BigClam &set_F(const std::vector<double> &F, const std::vector<double> *sumF = nullptr) {
         need();
         if ((int64_t)F.size() != n_ * K_) throw Error(BIGCLAM_EINVAL, "F must be n x K");
-        check(multi_ ? bigclam_multi_set_F(multi_, F.data()) : bigclam_set_F(ctx_, F.data()), "set_F");
-        if (sumF != nullptr) check(multi_ ? bigclam_multi_set_sumF(multi_, sumF->data()) : bigclam_set_sumF(ctx_, sumF->data()), "set_sumF");
+        call("set_F", bigclam_set_F, bigclam_multi_set_F, F.data());
+        if (sumF != nullptr) call("set_sumF", bigclam_set_sumF, bigclam_multi_set_sumF, sumF->data());
         return *this;
     }
     std::vector<double> F() {
@@ -169,8 +169,7 @@ public:
         if (Sbc.empty()) conductanceLocalMin();
         if (K != K_ || (ctx_ == nullptr && multi_ == nullptr)) set_K(K);
         const int32_t inc = include_self ? 1 : 0;
-        check(multi_ ? bigclam_multi_init_F(multi_, Sbc.data(), (int64_t)Sbc.size(), inc, pad_seed)
-                     : bigclam_init_F(ctx_, Sbc.data(), (int64_t)Sbc.size(), inc, pad_seed), "init_F");
+        call("init_F", bigclam_init_F, bigclam_multi_init_F, Sbc.data(), (int64_t)Sbc.size(), inc, pad_seed);
         return *this;
     }
     // initNeighborComF(K) (:81-108): builds F0 from the ranked seeds, loads it and returns it (n x K).
@@ -189,13 +188,13 @@ public:
         }
         double llh = 0.0;
         const uint8_t *m = uset != nullptr ? mask.data() : nullptr;
-        check(multi_ ? bigclam_multi_step(multi_, m, &llh, &last_n_updated) : bigclam_step(ctx_, m, &llh, &last_n_updated), "step");
+        call("step", bigclam_step, bigclam_multi_step, m, &llh, &last_n_updated);
         return llh;
     }
     double loglikelihood() {
         need();
         double llh = 0.0;
-        check(multi_ ? bigclam_multi_loglikelihood(multi_, &llh) : bigclam_loglikelihood(ctx_, &llh), "loglikelihood");
+        call("loglikelihood", bigclam_loglikelihood, bigclam_multi_loglikelihood, &llh);
         return llh;
     }
     // :225-243: one call for LLHold, then until |1 - new/old| < 1e-4; returns what the script returns (:242).
@@ -232,13 +231,11 @@ public:
     void extract_grouped(double delta, std::vector<int64_t> &comptr, std::vector<int32_t> &members, std::vector<int32_t> &zero_rows) {
         need();
         int64_t nnz = 0, z = 0;
-        check(multi_ ? bigclam_multi_extract_nnz(multi_, delta, &nnz, &z) : bigclam_extract_nnz(ctx_, delta, &nnz, &z), "extract");
+        call("extract", bigclam_extract_nnz, bigclam_multi_extract_nnz, delta, &nnz, &z);
         comptr.assign((size_t)K_ + 1, 0);
         members.assign((size_t)std::max<int64_t>(nnz, 1), 0);
         zero_rows.assign((size_t)std::max<int64_t>(z, 1), 0);
-        check(multi_ ? bigclam_multi_extract_grouped(multi_, delta, comptr.data(), members.data(), zero_rows.data())
-                     : bigclam_extract_grouped(ctx_, delta, comptr.data(), members.data(), zero_rows.data()),
-              "extract");
+        call("extract", bigclam_extract_grouped, bigclam_multi_extract_grouped, delta, comptr.data(), members.data(), zero_rows.data());
         members.resize((size_t)nnz);
         zero_rows.resize((size_t)z);
     }
@@ -259,9 +256,8 @@ public:
         s.internal.assign((size_t)K_, 0);
         s.conductance.assign((size_t)K_, 0.0);
         const int32_t zr = zero_rows_everywhere ? 1 : 0;
-        check(multi_ ? bigclam_multi_community_stats(multi_, delta, zr, s.size.data(), s.volume.data(), s.internal.data(), s.conductance.data())
-                     : bigclam_community_stats(ctx_, delta, zr, s.size.data(), s.volume.data(), s.internal.data(), s.conductance.data()),
-              "community_stats");
+        call("community_stats", bigclam_community_stats, bigclam_multi_community_stats, delta, zr, s.size.data(), s.volume.data(),
+             s.internal.data(), s.conductance.data());
         return s;
     }
 
@@ -293,11 +289,8 @@ public:
         double scores[3] = {0.0, 0.0, 0.0};
         const int32_t zr = zero_rows_everywhere ? 1 : 0;
         const int32_t *mp = members.empty() ? nullptr : members.data();
-        check(multi_ ? bigclam_multi_cover_scores(multi_, delta, zr, (int64_t)q, ptr.data(), mp, s.f1_detected.data(), s.match_detected.data(),
-                                                  s.f1_truth.data(), s.match_truth.data(), s.hcond_detected.data(), s.hcond_truth.data(), scores)
-                     : bigclam_cover_scores(ctx_, delta, zr, (int64_t)q, ptr.data(), mp, s.f1_detected.data(), s.match_detected.data(),
-                                            s.f1_truth.data(), s.match_truth.data(), s.hcond_detected.data(), s.hcond_truth.data(), scores),
-              "score_against");
+        call("score_against", bigclam_cover_scores, bigclam_multi_cover_scores, delta, zr, (int64_t)q, ptr.data(), mp, s.f1_detected.data(),
+             s.match_detected.data(), s.f1_truth.data(), s.match_truth.data(), s.hcond_detected.data(), s.hcond_truth.data(), scores);
         s.f1_truth.resize(q);
         s.hcond_truth.resize(q);
         s.match_truth.resize(q);
@@ -315,9 +308,7 @@ public:
         x.assign(u.size(), 0.0);
         p.assign(u.size(), 0.0);
         const int64_t cnt = (int64_t)u.size();
-        check(multi_ ? bigclam_multi_pair_affinity(multi_, u.data(), v.data(), cnt, x.data(), p.data())
-                     : bigclam_pair_affinity(ctx_, u.data(), v.data(), cnt, x.data(), p.data()),
-              "edge_probability");
+        call("edge_probability", bigclam_pair_affinity, bigclam_multi_pair_affinity, u.data(), v.data(), cnt, x.data(), p.data());
     }
     // For each query node (empty = all nodes) the m nodes at distance 2, not yet linked, with the largest affinity x > 0
     // (x descending, then id ascending): v and x are nodes.size() x m row-major, padded with -1 and 0 (bigclam_recommend).
@@ -327,9 +318,7 @@ public:
         const int32_t *q = nodes.empty() ? nullptr : nodes.data();
         v.assign((size_t)(cnt * std::max(m, 0)), -1);
         x.assign((size_t)(cnt * std::max(m, 0)), 0.0);
-        check(multi_ ? bigclam_multi_recommend(multi_, q, cnt, m, v.data(), x.data(), nullptr)
-                     : bigclam_recommend(ctx_, q, cnt, m, v.data(), x.data(), nullptr),
-              "recommend");
+        call("recommend", bigclam_recommend, bigclam_multi_recommend, q, cnt, m, v.data(), x.data(), nullptr);
     }
     // A graph sampled from the model (bigclam_sample_graph): pairs that share a component are edges with probability
     // p_uv (edge_probability's p), the others with probability eps; a symmetric CSR, rows ascending, the shape set_graph
@@ -337,13 +326,10 @@ public:
     void sample_graph(uint64_t seed, double eps, std::vector<int64_t> &rowptr, std::vector<int32_t> &col) {
         need();
         int64_t nnz = 0;
-        check(multi_ ? bigclam_multi_sample_graph_nnz(multi_, seed, eps, &nnz) : bigclam_sample_graph_nnz(ctx_, seed, eps, &nnz),
-              "sample_graph");
+        call("sample_graph", bigclam_sample_graph_nnz, bigclam_multi_sample_graph_nnz, seed, eps, &nnz);
         rowptr.assign((size_t)n_ + 1, 0);
         col.assign((size_t)std::max<int64_t>(nnz, 1), 0);
-        check(multi_ ? bigclam_multi_sample_graph(multi_, seed, eps, rowptr.data(), col.data())
-                     : bigclam_sample_graph(ctx_, seed, eps, rowptr.data(), col.data()),
-              "sample_graph");
+        call("sample_graph", bigclam_sample_graph, bigclam_multi_sample_graph, seed, eps, rowptr.data(), col.data());
         col.resize((size_t)nnz);
     }
     // Rows for new nodes with the fitted F and sumF held fixed (bigclam_fold_in): query node i has the neighbour list
@@ -357,19 +343,14 @@ public:
         const int64_t q = (int64_t)rowptr.size() - 1;
         if (rowptr.back() > (int64_t)col.size()) throw Error(BIGCLAM_EINVAL, "fold_in: rowptr goes beyond col");
         int64_t nnz = 0;
-        check(multi_ ? bigclam_multi_fold_in_nnz(multi_, q, rowptr.data(), col.data(), max_iter, rel_tol, &nnz)
-                     : bigclam_fold_in_nnz(ctx_, q, rowptr.data(), col.data(), max_iter, rel_tol, &nnz),
-              "fold_in");
+        call("fold_in", bigclam_fold_in_nnz, bigclam_multi_fold_in_nnz, q, rowptr.data(), col.data(), max_iter, rel_tol, &nnz);
         indptr.assign((size_t)q + 1, 0);
         indices.assign((size_t)std::max<int64_t>(nnz, 1), 0);
         values.assign((size_t)std::max<int64_t>(nnz, 1), 0.0);
         llh.assign((size_t)q, 0.0);
         iters.assign((size_t)q, 0);
-        check(multi_ ? bigclam_multi_fold_in(multi_, q, rowptr.data(), col.data(), max_iter, rel_tol, indptr.data(), indices.data(),
-                                             values.data(), llh.data(), iters.data())
-                     : bigclam_fold_in(ctx_, q, rowptr.data(), col.data(), max_iter, rel_tol, indptr.data(), indices.data(), values.data(),
-                                       llh.data(), iters.data()),
-              "fold_in");
+        call("fold_in", bigclam_fold_in, bigclam_multi_fold_in, q, rowptr.data(), col.data(), max_iter, rel_tol, indptr.data(), indices.data(),
+             values.data(), llh.data(), iters.data());
         indices.resize((size_t)nnz);
         values.resize((size_t)nnz);
     }
@@ -401,9 +382,7 @@ private:
         need();
         std::vector<double> trace(65536);
         double llh = 0.0;
-        check(multi_ ? bigclam_multi_run(multi_, variant, rel_tol, max_outer, &llh, &last_calls, trace.data(), (int64_t)trace.size())
-                     : bigclam_run(ctx_, variant, rel_tol, max_outer, &llh, &last_calls, trace.data(), (int64_t)trace.size()),
-              "run");
+        call("run", bigclam_run, bigclam_multi_run, variant, rel_tol, max_outer, &llh, &last_calls, trace.data(), (int64_t)trace.size());
         trace.resize((size_t)std::min<int64_t>(last_calls, (int64_t)trace.size()));
         last_trace = std::move(trace);
         return llh;
@@ -412,6 +391,11 @@ private:
         if (ctx_ == nullptr && multi_ == nullptr) throw Error(BIGCLAM_EINVAL, "no context: call set_graph()/load_edge_list() and set_K() first");
     }
     static std::string str(const char *s) { return s != nullptr ? s : "unknown error"; }
+    // The same C call on whichever handle this instance holds, its error thrown as an Error prefixed with `what`.
+    template <typename Single, typename Multi, typename... A>
+    void call(const char *what, Single single_fn, Multi multi_fn, A... args) const {
+        check(multi_ ? multi_fn(multi_, args...) : single_fn(ctx_, args...), what);
+    }
     void check(int rc, const char *what) const {
         if (rc == BIGCLAM_OK) return;
         const char *msg = multi_ ? bigclam_multi_last_error(multi_) : bigclam_last_error(ctx_);
