@@ -138,6 +138,10 @@ SIGNATURES = {
     "bigclam_multi_community_stats": (C.c_int, [_vp, _dbl, _i32, _vp, _vp, _vp, _vp]),
     "bigclam_cover_scores": (C.c_int, [_vp, _dbl, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigclam_multi_cover_scores": (C.c_int, [_vp, _dbl, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigclam_community_overlaps_nnz": (C.c_int, [_vp, _dbl, _i32, _pi64, _pi64]),
+    "bigclam_community_overlaps": (C.c_int, [_vp, _dbl, _i32, _vp, _vp, _vp, _vp]),
+    "bigclam_multi_community_overlaps_nnz": (C.c_int, [_vp, _dbl, _i32, _pi64, _pi64]),
+    "bigclam_multi_community_overlaps": (C.c_int, [_vp, _dbl, _i32, _vp, _vp, _vp, _vp]),
     "bigclam_conductance_seeds": (C.c_int, [_i64, _vp, _vp, _vp, _vp, _pi64]),
     "bigclam_conductance_seeds_gpu": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _vp, _pi64]),
     "bigclam_init_neighbor_com_F": (C.c_int, [_i64, _vp, _vp, _i32, _vp, _i64, _i32, C.c_uint64, _vp]),

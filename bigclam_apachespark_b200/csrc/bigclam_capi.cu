@@ -2629,6 +2629,128 @@ extern "C" int bigclam_cover_scores(bigclam_ctx *ctx, double delta, int32_t zero
     return BIGCLAM_OK;
 }
 
+// Community overlaps (bigclam_b200.h, bigclam_community_overlaps).  The count pass gives |M_c|, z, row_fmax and the
+// F >= 0 check; the column index of the memberships (columns < k, so no zero row) gives each community's member list;
+// community_overlaps_kernel<false> every row's entry count, <true> the rows themselves, in ranges.
+struct OverlapPlan {
+    std::vector<int64_t> ptr;          // the count pass's column scan (k + 2)
+    std::vector<int64_t> ovptr;        // the output's row scan (k + 1)
+    DevBuf<double> fmax;
+    DevBuf<int64_t> colptr;
+    DevBuf<int32_t> members;
+    OverlapArgs a{};
+};
+
+static int overlaps_args_check(bigclam_ctx *ctx, const char *what, double delta, int32_t min_shared, const void *out1,
+                               const void *out2, const void *out3) {
+    if (!(delta > 0.0)) return fail(ctx, BIGCLAM_EINVAL, "%s: delta = %g, must be > 0", what, delta);
+    if (min_shared < 1) return fail(ctx, BIGCLAM_EINVAL, "%s: min_shared = %d, must be >= 1", what, min_shared);
+    if (out1 == nullptr || out2 == nullptr || out3 == nullptr) return fail(ctx, BIGCLAM_EINVAL, "%s: NULL output", what);
+    return BIGCLAM_OK;
+}
+
+static int overlaps_count(bigclam_ctx *ctx, const char *what, double delta, int32_t min_shared, OverlapPlan &pl) {
+    const int64_t n = ctx->n;
+    const int32_t k = ctx->p.k;
+    pl.ovptr.assign((size_t)k + 1, 0);
+    if (n == 0) {
+        pl.ptr.assign((size_t)k + 2, 0);
+        return BIGCLAM_OK;
+    }
+    CU(cudaSetDevice(ctx->device));
+    if (pl.fmax.reserve((size_t)n) != cudaSuccess) return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for %lld bytes of scratch", what, (long long)(8 * n));
+    if (int rc = extract_count(ctx, what, delta, pl.ptr, pl.fmax.p)) return rc;
+    const int64_t nm = pl.ptr[(size_t)k];
+    DevBuf<unsigned long long> cpos;
+    DevBuf<unsigned int> rowcnt;
+    if (pl.colptr.reserve((size_t)k + 1) != cudaSuccess || pl.members.reserve((size_t)nm) != cudaSuccess ||
+        cpos.reserve((size_t)k) != cudaSuccess || rowcnt.reserve((size_t)k) != cudaSuccess)
+        return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for the column index of %lld memberships", what, (long long)nm);
+    const RowSrc s = row_src(ctx);
+    const std::vector<unsigned long long> hpos(pl.ptr.begin(), pl.ptr.begin() + k);
+    CU(cudaMemcpyAsync(pl.colptr.p, pl.ptr.data(), sizeof(int64_t) * ((size_t)k + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(cpos.p, hpos.data(), sizeof(unsigned long long) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
+    const int wpb = 4;
+    colidx_kernel<true, MemberPred><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, 0, ctx->stream>>>(s, n, MemberPred{delta, k, nullptr}, 0, k,
+                                                                                        nullptr, cpos.p, pl.members.p);
+    CU(cudaGetLastError());
+    const size_t smem = sizeof(unsigned int) * (size_t)k;
+    CU(cudaFuncSetAttribute(community_overlaps_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(community_overlaps_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    pl.a = OverlapArgs{s, pl.fmax.p, pl.colptr.p, pl.members.p, delta, (unsigned int)min_shared, 0, rowcnt.p, nullptr, 0, nullptr, nullptr};
+    community_overlaps_kernel<false><<<(unsigned)k, 32 * kOverlapWarps, smem, ctx->stream>>>(pl.a);
+    CU(cudaGetLastError());
+    std::vector<unsigned int> hcnt((size_t)k);
+    CU(cudaMemcpyAsync(hcnt.data(), rowcnt.p, sizeof(unsigned int) * (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    pl.a.rowcnt = nullptr;
+    for (int32_t c = 0; c < k; ++c) pl.ovptr[(size_t)c + 1] = pl.ovptr[(size_t)c] + hcnt[(size_t)c];
+    return BIGCLAM_OK;
+}
+
+extern "C" int bigclam_community_overlaps_nnz(bigclam_ctx *ctx, double delta, int32_t min_shared, int64_t *nnz_out, int64_t *n_zero_rows_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_community_overlaps_nnz";
+    if (int rc = overlaps_args_check(ctx, what, delta, min_shared, nnz_out, n_zero_rows_out, nnz_out)) return rc;
+    OverlapPlan pl;
+    if (int rc = overlaps_count(ctx, what, delta, min_shared, pl)) return rc;
+    const int32_t k = ctx->p.k;
+    *nnz_out = pl.ovptr[(size_t)k];
+    *n_zero_rows_out = pl.ptr[(size_t)k + 1] - pl.ptr[(size_t)k];
+    return BIGCLAM_OK;
+}
+
+// Count, then the rows in consecutive ranges of communities whose output fits the scratch bound (a longer row gets a
+// range of its own): fill, copy out.
+extern "C" int bigclam_community_overlaps(bigclam_ctx *ctx, double delta, int32_t min_shared, int64_t *ovptr_out, int32_t *other_out,
+                                          int32_t *shared_out, int64_t *size_out) {
+    if (ctx == nullptr) return BIGCLAM_EINVAL;
+    const char *what = "bigclam_community_overlaps";
+    if (int rc = overlaps_args_check(ctx, what, delta, min_shared, ovptr_out, other_out, shared_out)) return rc;
+    OverlapPlan pl;
+    if (int rc = overlaps_count(ctx, what, delta, min_shared, pl)) return rc;
+    const int32_t k = ctx->p.k;
+    const std::vector<int64_t> &ov = pl.ovptr;
+    std::copy(ov.begin(), ov.end(), ovptr_out);
+    if (size_out != nullptr)
+        for (int32_t c = 0; c < k; ++c) size_out[c] = pl.ptr[(size_t)c + 1] - pl.ptr[(size_t)c];
+    if (ov[(size_t)k] == 0) return BIGCLAM_OK;
+    int64_t budget;
+    CU(extract_budget(budget));
+    const int64_t budget_entries = std::max<int64_t>(1, budget / (int64_t)(2 * sizeof(int32_t)));
+    const size_t smem = sizeof(unsigned int) * (size_t)k;
+    DevBuf<int64_t> dov;
+    DevBuf<int32_t> dother, dshared;
+    CU(dov.reserve((size_t)k + 1));
+    CU(cudaMemcpyAsync(dov.p, ov.data(), sizeof(int64_t) * ((size_t)k + 1), cudaMemcpyHostToDevice, ctx->stream));
+    for (int32_t c0 = 0; c0 < k;) {
+        int32_t c1 = c0 + 1;
+        while (c1 < k && ov[(size_t)c1 + 1] - ov[(size_t)c0] <= budget_entries) ++c1;
+        const int64_t base = ov[(size_t)c0], total = ov[(size_t)c1] - base;
+        if (total > 0) {
+            if (dother.reserve((size_t)total) != cudaSuccess || dshared.reserve((size_t)total) != cudaSuccess) {
+                if (c1 - c0 == 1)
+                    return fail(ctx, BIGCLAM_ENOMEM, "%s: community %d overlaps %lld communities; no room for them", what, c0, (long long)total);
+                return fail(ctx, BIGCLAM_ENOMEM, "%s: no room for a %lld-byte range of communities %d..%d", what,
+                            (long long)(total * (int64_t)(2 * sizeof(int32_t))), c0, c1 - 1);
+            }
+            OverlapArgs a = pl.a;
+            a.c0 = c0;
+            a.ovptr = dov.p + c0;
+            a.base = base;
+            a.other = dother.p;
+            a.shared = dshared.p;
+            community_overlaps_kernel<true><<<(unsigned)(c1 - c0), 32 * kOverlapWarps, smem, ctx->stream>>>(a);
+            CU(cudaGetLastError());
+            CU(cudaMemcpyAsync(other_out + base, dother.p, sizeof(int32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaMemcpyAsync(shared_out + base, dshared.p, sizeof(int32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaStreamSynchronize(ctx->stream));
+        }
+        c0 = c1;
+    }
+    return BIGCLAM_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Fused collective of the node-partitioned path: exchange buffers (see bigclam_ctx::x_*).
 static int xchg_alloc(bigclam_ctx *ctx, int32_t world, int32_t rank) {
@@ -2884,6 +3006,14 @@ extern "C" int bigclam_multi_cover_scores(bigclam_multi *m, double delta, int32_
                                           int32_t *match_truth, double *hcond_det, double *hcond_truth, double *scores_out) {
     return on_rank(m, 0, bigclam_cover_scores, delta, zero_rows, q, truth_ptr, truth_members, f1_det, match_det, f1_truth, match_truth,
                    hcond_det, hcond_truth, scores_out);
+}
+extern "C" int bigclam_multi_community_overlaps_nnz(bigclam_multi *m, double delta, int32_t min_shared, int64_t *nnz_out,
+                                                    int64_t *n_zero_rows_out) {
+    return on_rank(m, 0, bigclam_community_overlaps_nnz, delta, min_shared, nnz_out, n_zero_rows_out);
+}
+extern "C" int bigclam_multi_community_overlaps(bigclam_multi *m, double delta, int32_t min_shared, int64_t *ovptr_out, int32_t *other_out,
+                                                int32_t *shared_out, int64_t *size_out) {
+    return on_rank(m, 0, bigclam_community_overlaps, delta, min_shared, ovptr_out, other_out, shared_out, size_out);
 }
 
 extern "C" int bigclam_multi_loglikelihood(bigclam_multi *m, double *llh_out) {

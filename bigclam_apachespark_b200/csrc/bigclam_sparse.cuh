@@ -1591,6 +1591,31 @@ __global__ void community_stats_kernel(RowSrc s, const int64_t *__restrict__ row
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// The member-counting loop of cover_scores_kernel and community_overlaps_kernel: the warps of a block walk the rows
+// list[i0, i1), one row per warp (warp w of kWarps takes i0 + w, i0 + w + kWarps, ...), and add 1 to cnt[c] (shared
+// memory) for each c in M(u), read with row_view + is_member; fmax[u] = row_fmax from the count pass.  A zero row
+// (fmax 0) is never expanded: the returned value (the same on every lane) is the number of zero rows the warp met.
+template <int kWarps>
+__device__ __forceinline__ unsigned int count_memberships(const RowSrc &s, const double *__restrict__ fmax, double delta,
+                                                          const int32_t *__restrict__ list, int64_t i0, int64_t i1,
+                                                          unsigned int *cnt) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned int zeros = 0;
+    for (int64_t i = i0 + warp; i < i1; i += kWarps) {
+        const int32_t u = list[i];
+        const double fu = fmax[u];
+        if (fu == 0.0) {                                     // (warp-uniform)
+            ++zeros;
+            continue;
+        }
+        const RowView r = row_view(s, u);
+        for (int j = lane; j < r.cnt; j += 32)
+            if (is_member(r.vals[j], fu, delta)) atomicAdd(&cnt[r.idx != nullptr ? (int)r.idx[j] : j], 1u);
+    }
+    return zeros;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Cover scores (bigclam_cover_scores): the detected cover X (the communities of is_member, the zero rows in every
 // community or in none) against a truth cover Y given as a CSR of distinct members.  Non-negative doubles order as their
 // bits, so the per-community maxima and minima over t are 64-bit integer atomics and come out the same in any order.
@@ -1631,9 +1656,9 @@ struct CoverArgs {
     int32_t *match_t;                  // per t: the smallest c attaining f1_t, -1 when f1_t = 0
 };
 
-// One block per truth community t (empty ones return).  The warps walk t's members u, one member per warp: a zero row
-// adds 1 to z_t, any other row adds 1 to cnt[c] (k counters in shared memory) for each c in M(u), read with row_view +
-// is_member as community_stats_kernel does, so zero rows are never expanded.  Then every non-empty c is a pair (c, t)
+// One block per truth community t (empty ones return).  count_memberships walks t's members u: a zero row adds 1 to
+// z_t, any other row adds 1 to cnt[c] (k counters in shared memory) for each c in M(u), so zero rows are never
+// expanded.  Then every non-empty c is a pair (c, t)
 // with a = cnt[c] (+ z_t when zero_rows), x = xs[c], y = |Y_t|:
 //   !kTies  F1 = 2a / (x + y) goes to f1_det[c] (atomicMax on its bits, after a read that skips what cannot improve)
 //           and to the block's maximum (smallest c on ties); an admissible pair's H(X_c | Y_t) goes to hc_det[c]
@@ -1656,17 +1681,8 @@ __global__ void __launch_bounds__(32 * kCoverWarps) cover_scores_kernel(CoverArg
     for (int c = threadIdx.x; c < k; c += blockDim.x) cnt[c] = 0u;
     if (threadIdx.x == 0) s_zt = 0u;
     __syncthreads();
-    for (int64_t i = m0 + warp; i < m1; i += kCoverWarps) {
-        const int32_t u = a.tmem[i];
-        const double fu = a.fmax[u];
-        if (fu == 0.0) {                                     // (warp-uniform)
-            if (lane == 0) atomicAdd(&s_zt, 1u);
-            continue;
-        }
-        const RowView r = row_view(a.s, u);
-        for (int j = lane; j < r.cnt; j += 32)
-            if (is_member(r.vals[j], fu, a.delta)) atomicAdd(&cnt[r.idx != nullptr ? (int)r.idx[j] : j], 1u);
-    }
+    const unsigned int zeros = count_memberships<kCoverWarps>(a.s, a.fmax, a.delta, a.tmem, m0, m1, cnt);
+    if (lane == 0 && zeros != 0u) atomicAdd(&s_zt, zeros);
     __syncthreads();
     const int64_t n = a.n, y = m1 - m0, zt = a.zero_rows ? (int64_t)s_zt : 0;
     const double *h = a.h;
@@ -1727,6 +1743,66 @@ __global__ void __launch_bounds__(32 * kCoverWarps) cover_scores_kernel(CoverArg
     a.match_t[t] = best > 0.0 ? bc : -1;
     a.hc_t[t] = hmin;
     a.hy_t[t] = hy;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Community overlaps (bigclam_community_overlaps): shared(c, d) = |M_c ∩ M_d| over the non-zero rows, for every pair
+// c != d with shared(c, d) >= min_shared.
+struct OverlapArgs {
+    RowSrc s;
+    const double *fmax;                // row_fmax from the count pass
+    const int64_t *colptr;             // the column index of the memberships (colidx_kernel with MemberPred, columns < k:
+    const int32_t *members;            //   no zero rows), any order within a column
+    double delta;
+    unsigned int min_shared;
+    int32_t c0;                        // block b works on community c0 + b
+    unsigned int *rowcnt;              // count launch: rowcnt[c] = the entries of row c
+    const int64_t *ovptr;              // fill launch: row c goes to other / shared [ovptr[c - c0] - base, ...)
+    int64_t base;
+    int32_t *other, *shared;
+};
+
+// One block per community c.  count_memberships walks c's members u and adds 1 to cnt[d] (k counters in shared memory)
+// for each d in M(u), so cnt[d] = shared(c, d) (cnt[c] = |M_c|).  Then one block-wide ordered compaction over the
+// counters, blockDim.x of them per round: a ballot per warp, the warps' totals in shared memory, a running offset.  The
+// count launch (!kFill) keeps the total, the fill launch writes each kept d and its count at its rank, so every row
+// comes out ascending in d with no sort.  Everything is integer: any order of the atomics gives the same output.
+constexpr int kOverlapWarps = 8;
+template <bool kFill>
+__global__ void __launch_bounds__(32 * kOverlapWarps) community_overlaps_kernel(OverlapArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    __shared__ unsigned int s_wsum[kOverlapWarps];
+    unsigned int *cnt = reinterpret_cast<unsigned int *>(smem_raw);
+    const int c = a.c0 + (int)blockIdx.x;
+    const int k = a.s.k, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int d = threadIdx.x; d < k; d += blockDim.x) cnt[d] = 0u;
+    __syncthreads();
+    count_memberships<kOverlapWarps>(a.s, a.fmax, a.delta, a.members, a.colptr[c], a.colptr[c + 1], cnt);
+    __syncthreads();
+    const int64_t out0 = kFill ? a.ovptr[c - a.c0] - a.base : 0;
+    unsigned int done = 0;                                   // (block-uniform) entries kept in the rounds before
+    for (int d0 = 0; d0 < k; d0 += blockDim.x) {
+        const int d = d0 + (int)threadIdx.x;
+        const unsigned int v = d < k ? cnt[d] : 0u;
+        const bool keep = d < k && d != c && v >= a.min_shared;
+        const unsigned int m = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) s_wsum[warp] = (unsigned int)__popc(m);
+        __syncthreads();
+        unsigned int before = 0, round = 0;
+        for (int w = 0; w < kOverlapWarps; ++w) {
+            const unsigned int x = s_wsum[w];
+            before += w < warp ? x : 0u;
+            round += x;
+        }
+        if (kFill && keep) {
+            const int64_t p = out0 + done + before + (unsigned int)__popc(m & ((1u << lane) - 1u));
+            a.other[p] = d;
+            a.shared[p] = (int32_t)v;
+        }
+        done += round;
+        __syncthreads();                                     // (s_wsum is rewritten by the next round)
+    }
+    if (!kFill && threadIdx.x == 0) a.rowcnt[c] = done;
 }
 
 struct SampleArgs {

@@ -460,6 +460,30 @@ class BigClam:
                     match_detected=match_det, f1_truth=f1_truth[:q], match_truth=match_truth[:q], hcond_detected=hc_det,
                     hcond_truth=hc_truth[:q])
 
+    def community_overlaps(self, delta, min_shared=1, zero_rows_everywhere=True):
+        """How the communities of extract_communities(delta) overlap each other, on the GPU (bigclam_community_overlaps,
+        whose header comment defines the counts).  Lists, for every community c, the communities d != c that share at
+        least min_shared non-zero rows with it.  Returns dict(ptr int64[K + 1], other int32[nnz], shared int32[nnz],
+        size int64[K], jaccard float64[nnz], zero_rows=z): row c is other[ptr[c]:ptr[c + 1]] (ascending) with the shared
+        members and the Jaccard index shared / (size_c + size_d - shared) of each pair; the output is symmetric.
+        zero_rows_everywhere: the z all-zero rows are in every community (as coded) or in none.  As coded, shared and
+        size include z, and a pair that is not listed still shares the z zero rows; min_shared always applies to the
+        non-zero rows alone."""
+        delta, min_shared = float(delta), int(min_shared)
+        nnz, z = C.c_int64(), C.c_int64()
+        self._call("community_overlaps_nnz", delta, min_shared, C.byref(nnz), C.byref(z))
+        K = self.K
+        ptr, size = np.zeros(K + 1, dtype=np.int64), np.zeros(K, dtype=np.int64)
+        other, shared = np.empty(max(nnz.value, 1), dtype=np.int32), np.empty(max(nnz.value, 1), dtype=np.int32)
+        self._call("community_overlaps", delta, min_shared, ptr.ctypes.data, other.ctypes.data, shared.ctypes.data, size.ctypes.data)
+        other, shared = other[:nnz.value], shared[:nnz.value]
+        if zero_rows_everywhere and z.value:
+            shared = shared + np.int32(z.value)                 # shared + z <= n < 2^31
+            size = size + z.value
+        rows = np.repeat(np.arange(K), np.diff(ptr))
+        jaccard = shared / (size[rows] + size[other] - shared)
+        return dict(ptr=ptr, other=other, shared=shared, size=size, jaccard=jaccard, zero_rows=int(z.value))
+
     # ---- diagnostics ----
     def accepted(self) -> np.ndarray:
         out = np.empty(self.n, dtype=np.int8)

@@ -391,6 +391,43 @@ int bigclam_multi_cover_scores(bigclam_multi *m, double delta, int32_t zero_rows
                                int32_t *match_truth, double *hcond_det, double *hcond_truth, double *scores_out);
 
 /*
+ * How the communities of the current F overlap each other: the shared members of every overlapping pair.
+ *
+ * Membership is the rule above (delta > 0 and not NaN, +inf allowed; F >= 0).  M_c is the set of NON-ZERO rows that are
+ * members of community c, and z the number of all-zero rows; as coded, each of those is a member of every community.
+ * For c != d:
+ *   shared(c, d) = |M_c ∩ M_d|          (non-zero rows only)
+ * The output lists, for every community c, the communities d != c with shared(c, d) >= min_shared (min_shared >= 1),
+ * as a CSR over communities: ovptr_out (k + 1, int64), other_out (nnz, int32, d ascending within a row) and shared_out
+ * (nnz, int32, shared(c, d)).  It is symmetric (d is in row c exactly when c is in row d, with the same count) and never
+ * lists the diagonal.  size_out (k, int64, optional) gets |M_c|, and bigclam_community_overlaps_nnz's n_zero_rows_out
+ * gets z.  Zero rows are kept out of every count and reported once, as bigclam_extract_grouped reports them, so the
+ * caller decides what they mean:
+ *   as coded (zero rows in every community): a pair's intersection is shared + z and a size is |M_c| + z; a pair that
+ *     is not listed still shares the z zero rows;
+ *   zero rows in no community: both are taken as they are.
+ * Every number is an exact integer, and the output depends on (F bits, delta, min_shared) only: not on the row layout,
+ * the range cut, the number of GPUs or the device.
+ *
+ * bigclam_community_overlaps_nnz gives nnz and z; bigclam_community_overlaps fills the outputs (sized with them; it
+ * counts again, nothing is kept between the calls).  BIGCLAM_EINVAL before any device work for delta <= 0 or NaN,
+ * min_shared < 1 or a NULL required output (other_out and shared_out also for nnz = 0); a negative entry of F gives
+ * BIGCLAM_EUNSUPPORTED naming the smallest such row; n = 0 gives zeros.  Device scratch is O(n + k + the memberships of
+ * the non-zero rows), nothing n x k; the rows are filled in consecutive ranges of communities whose output stays within
+ * the smaller of 1 GiB and 10 % of the free device memory (a row has at most k - 1 entries, so a range always holds
+ * one); BIGCLAM_ENOMEM, naming the community, when even one row's room cannot be allocated.  Reads F only (no state
+ * changes: F, sumF, accepted indices, a speculative step), on the context's stream, synchronous.  The cost of a pass is
+ * sum over the non-zero rows u of m_u^2 (m_u = the communities u is in) shared-memory increments, plus O(k) per
+ * community.  The multi-GPU calls read rank 0's replica; their errors go to bigclam_multi_last_error.
+ */
+int bigclam_community_overlaps_nnz(bigclam_ctx *ctx, double delta, int32_t min_shared, int64_t *nnz_out, int64_t *n_zero_rows_out);
+int bigclam_community_overlaps(bigclam_ctx *ctx, double delta, int32_t min_shared, int64_t *ovptr_out /* k + 1 */, int32_t *other_out /* nnz */,
+                               int32_t *shared_out /* nnz */, int64_t *size_out /* k, optional */);
+int bigclam_multi_community_overlaps_nnz(bigclam_multi *m, double delta, int32_t min_shared, int64_t *nnz_out, int64_t *n_zero_rows_out);
+int bigclam_multi_community_overlaps(bigclam_multi *m, double delta, int32_t min_shared, int64_t *ovptr_out, int32_t *other_out,
+                                     int32_t *shared_out, int64_t *size_out);
+
+/*
  * The fitted model as a model of edges (the clamp of bigclam4-7.scala:166, the edge term of :218), on the current F:
  *   x_uv = sum of F_uc * F_vc over the components c that are non-zero in both rows, folded left in ascending c with
  *          every product and every sum rounded on its own (the same bits for sparse and dense rows and for (v, u));

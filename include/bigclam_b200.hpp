@@ -19,6 +19,8 @@
 //                                                                extract_grouped(delta, ...)
 //   community scores, the formula of conductanceLocalMin :64-67  community_stats(delta, zero_rows_everywhere)
 //   Avg-F1 (thesis p.21) and overlapping NMI against a known cover  score_against(truth, delta, zero_rows_everywhere)
+//   the shared members of every overlapping pair of communities  community_overlaps(delta, min_shared,
+//                                                                zero_rows_everywhere)
 //   the model P(u,v) = 1 - exp(-F_u.F_v), clamp of :166          edge_probability(u, v), recommend(nodes, m),
 //                                                                sample_graph(seed, eps)
 //   rows for new nodes, the fit held fixed (:157-184 per node)    fold_in(rowptr, col, max_iter, rel_tol, ...)
@@ -297,6 +299,42 @@ public:
         s.avg_f1 = scores[0];
         s.nmi_lfk = scores[1];
         s.nmi_max = scores[2];
+        return s;
+    }
+
+    // How the communities of extract(delta) overlap each other (bigclam_community_overlaps, whose header comment defines
+    // the counts): row c lists other[ptr[c] .. ptr[c + 1]) ascending, the communities d != c sharing at least min_shared
+    // non-zero rows with c, with the shared members and the Jaccard index shared / (size_c + size_d - shared) of each
+    // pair; symmetric.  zero_rows_everywhere: the zero_rows all-zero rows are in every community (as coded: shared and
+    // size include them, and a pair that is not listed still shares them) or in none.  Works for multi-GPU handles too.
+    struct CommunityOverlaps {
+        std::vector<int64_t> ptr, size;
+        std::vector<int32_t> other, shared;
+        std::vector<double> jaccard;
+        int64_t zero_rows = 0;
+    };
+    CommunityOverlaps community_overlaps(double delta, int32_t min_shared = 1, bool zero_rows_everywhere = true) {
+        need();
+        int64_t nnz = 0;
+        CommunityOverlaps s;
+        call("community_overlaps", bigclam_community_overlaps_nnz, bigclam_multi_community_overlaps_nnz, delta, min_shared, &nnz, &s.zero_rows);
+        s.ptr.assign((size_t)K_ + 1, 0);
+        s.size.assign((size_t)K_, 0);
+        s.other.assign((size_t)std::max<int64_t>(nnz, 1), 0);
+        s.shared.assign((size_t)std::max<int64_t>(nnz, 1), 0);
+        call("community_overlaps", bigclam_community_overlaps, bigclam_multi_community_overlaps, delta, min_shared, s.ptr.data(),
+             s.other.data(), s.shared.data(), s.size.data());
+        s.other.resize((size_t)nnz);
+        s.shared.resize((size_t)nnz);
+        const int64_t z = zero_rows_everywhere ? s.zero_rows : 0;
+        for (auto &x : s.shared) x += (int32_t)z;
+        for (auto &x : s.size) x += z;
+        s.jaccard.resize((size_t)nnz);
+        for (int c = 0; c < K_; ++c)
+            for (int64_t i = s.ptr[(size_t)c]; i < s.ptr[(size_t)c + 1]; ++i) {
+                const int64_t a = s.shared[(size_t)i];
+                s.jaccard[(size_t)i] = (double)a / (double)(s.size[(size_t)c] + s.size[(size_t)s.other[(size_t)i]] - a);
+            }
         return s;
     }
 
