@@ -101,6 +101,10 @@ struct bigclam_ctx {
     unsigned int stats_seen[2] = {0u, 0u};        // d_stats at the last look (maybe_retile)
     unsigned int stats_read[2] = {0u, 0u};        // d_stats at the last bigclam_get_tile_stats
     unsigned int *d_stats = nullptr;              // [tiles on the tile path, tiles that fell back, nodes line-searched, nodes that asked for it]
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+    unsigned long long *d_phase_clocks = nullptr; // kTlPcBuckets x kTlPcSlots per resident warp (bigclam_phase_clocks)
+    size_t phase_clocks_n = 0;
+#endif
     unsigned int ls_read[2] = {0u, 0u};           // d_stats[2..3] at the last bigclam_get_ls_stats
     int ls_level = 1;                             // bounds on the tile path (1); 2 = on the general path too (BIGCLAM_LS_PRUNE=2: pays off only
                                                   // where most nodes have stopped moving AND the general path matters, e.g. com-amazon K=500: -4 %;
@@ -220,6 +224,9 @@ static void free_ctx(bigclam_ctx *c) {
     cudaFree(c->d_pool_top); cudaFree(c->d_overflow);
     cudaFree(c->d_node_llh); cudaFree(c->d_dcnt); cudaFree(c->d_block_part); cudaFree(c->d_ticket);
     cudaFree(c->d_tiles); cudaFree(c->d_tcol); cudaFree(c->d_stats); cudaFree(c->d_wide_scratch);
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+    cudaFree(c->d_phase_clocks);
+#endif
     if (c->x_ipc)
         for (int r = 0; r < c->x_world; ++r)
             if (r != c->x_rank) {
@@ -1259,6 +1266,18 @@ static int timed_launch(bigclam_ctx *ctx, const StepArgs &a, bool is_step) {
         sp.pr_kinv = std::nextafterf((float)(1.0 / (1.0 - ctx->p.max_p)), INFINITY) * 1.000001f;
         sp.pr_cap = std::nextafterf((float)(a.t_hi - a.t_lo), INFINITY) * 1.000001f;
         sp.wide_scratch = ctx->d_wide_scratch;
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+        {
+            const size_t nc = (size_t)ctx->sp_grid * ctx->sp_wpb * kTlPcBuckets * kTlPcSlots;
+            if (ctx->phase_clocks_n < nc) {
+                cudaFree(ctx->d_phase_clocks);
+                CU(cudaMalloc(&ctx->d_phase_clocks, nc * sizeof(unsigned long long)));
+                CU(cudaMemset(ctx->d_phase_clocks, 0, nc * sizeof(unsigned long long)));
+                ctx->phase_clocks_n = nc;
+            }
+            sp.phase_clocks = ctx->d_phase_clocks;
+        }
+#endif
         const bool hub = a.n_hub_items > 0, push = sp.n_peers > 0;
         const int threads = 32 * ctx->sp_wpb;
         if (ctx->wide) {
@@ -1644,6 +1663,24 @@ extern "C" int bigclam_get_tile_stats(bigclam_ctx *ctx, int64_t *tiles_done, int
     if (n_split_hubs) *n_split_hubs = ctx->sparse ? ctx->n_hubs : 0;
     return BIGCLAM_OK;
 }
+
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+// Phase profile (builds with BIGCLAM_TL_PHASE_CLOCKS only, tools/phase_clocks.py): out[kTlPcBuckets * kTlPcSlots] = the
+// counters summed over the warps since the last call; they start again from zero.
+extern "C" int bigclam_phase_clocks(bigclam_ctx *ctx, unsigned long long *out) {
+    if (ctx == nullptr || out == nullptr) return BIGCLAM_EINVAL;
+    const int nb = kTlPcBuckets * kTlPcSlots;
+    for (int i = 0; i < nb; ++i) out[i] = 0ull;
+    if (ctx->d_phase_clocks == nullptr) return BIGCLAM_OK;
+    CU(cudaSetDevice(ctx->device));
+    CU(cudaStreamSynchronize(ctx->stream));
+    std::vector<unsigned long long> h(ctx->phase_clocks_n);
+    CU(cudaMemcpy(h.data(), ctx->d_phase_clocks, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < h.size(); ++i) out[i % nb] += h[i];
+    CU(cudaMemset(ctx->d_phase_clocks, 0, h.size() * sizeof(unsigned long long)));
+    return BIGCLAM_OK;
+}
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // Node-partitioned pieces (DESIGN.md (e)).

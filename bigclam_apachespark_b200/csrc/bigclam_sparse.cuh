@@ -112,6 +112,9 @@ struct SparseArgs {
     int32_t ls_prune;
     float pr_xlo, pr_kinv, pr_cap;     // x_lo rounded down, 1 / (1 - MAX_P_) and S_hi - S_lo rounded up
     unsigned char *wide_scratch;       // wide rows: sp_wide_warp_bytes(ld) per resident warp, all zero between launches
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+    unsigned long long *phase_clocks;  // phase profile of the tile path (bigclam_tile.cuh, kTlPcBuckets)
+#endif
 };
 
 // The dense per-warp vectors are padded to a multiple of 32 components (zeros: a padding component has

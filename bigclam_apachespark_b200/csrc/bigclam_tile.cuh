@@ -86,13 +86,14 @@ static_assert(2 * kTlOwn16 < 255, "own-entry indices of the slots are bytes (0xf
 
 // The warp region of the tile path.  Buffers whose lifetimes do not overlap share bytes (phases: TlWarp::run):
 //   stageN   neighbour rows  A-I                  | xs (edge x trial)  J-K
-//   gd       tmask | pref_t (48 B per mask word of a node)  A-C2 | g per slot  G-H
-//            | g of the active components [kTlAct]  H-L; behind them we2  H2, fu on its way to fa  I, ent_val  I-J
+//   gd       tmask | pref_t (48 B per mask word of a node), behind them desc (u16 per entry)  A-C2 | g per slot  G-H2
+//            | g of the active components [kTlAct]  compaction-L; behind them fu on its way to fa  I, ent_val  I-J
 //   stageO   own rows  A-I (fu through slot_o, then through fo)   | fa (fu of the active components [kTlAct])  I-L
-//   slot_c   component of a slot  C2-L (below A only after H)     | ent_e, ent_a behind kTlAct  I-J
-//   slot_o   own-entry index of a slot (byte)  C2-H               | amap (slot -> active index, byte)  H-I   | plist  J
+//   slot_c   component of a slot  C2-L (below A only after the compaction)  | ent_e, ent_a behind kTlAct  I-J
+//   slot_o   own-entry index of a slot (byte)  C2-H2              | amap (slot -> active index, byte)  compaction-I  | plist  J
 //   erow, e_soff, e_cnt, e_io2 (entry -> row, rows' places)  A-I                                          | plist  J
-//   tail     we  D-G | fo (own-entry index of an active component, byte)  H-I | lcnt (byte)  I
+//   tail     we  D-G | we2  H2 | fo (own-entry index of an active component, byte)  compaction-I | lcnt (byte)  I
+// The compaction (active components to the front) runs after H2, and only in a tile with a line-searched node.
 // (sumF - fu of an active component is computed where phase J reads it.)
 constexpr int kTlOffG = 16 * kTlStage16;
 constexpr int kTlOffOwn = kTlOffG + 8 * kTlSlots;
@@ -103,18 +104,19 @@ constexpr int kTlOffErow = kTlOffAmap + kTlSlots;
 constexpr int kTlOffESoff = kTlOffErow + kTlErow;                     // e_soff, e_cnt [40 u16 each: 32 edges, then 8 nodes]
 constexpr int kTlOffEIo2 = kTlOffESoff + 2 * 2 * 40;
 constexpr int kTlOffEpos = kTlOffEIo2 + 2 * 32;
-constexpr int kTlOffENi = kTlOffEpos + 2 * 34;
-constexpr int kTlOffNu = (kTlOffENi + 32 + 3) & ~3;                   // n_u [8 int]
-constexpr int kTlOffNes = kTlOffNu + 4 * kTlMaxNodes;                 // n_es, n_sb, n_ab [12 u16 each], n_m [8], n_q [16], n_sv [8]
+constexpr int kTlOffNu = (kTlOffEpos + 2 * 34 + 32 + 3) & ~3;        // n_u [8 int] (32 bytes spare before it)
+constexpr int kTlOffNes = kTlOffNu + 4 * kTlMaxNodes;                 // n_es, n_sb (n_sb[nn]: all slots), n_ab [12 u16 each], n_m [8], n_q [16], n_sv [8]
 constexpr int kTlOffNjs = kTlOffNes + 2 * (12 + 12 + 12 + 8 + 16 + 8); // n_js, n_want, n_sl [8 bytes each], n_cnt [2]
 constexpr int kTlOffTail = (kTlOffNjs + 3 * 8 + 2 + 7) & ~7;
 constexpr int kTlTail = 8 * kTlMaxEdges;                              // we: one double per edge
 static_assert(8 * kTlAct + 8 * kTlEnt <= 8 * kTlSlots, "ent_val fits in gd behind the gradients of the active components");
-static_assert((4 + 2) * kTlMaxNodes * (kSpWideLd / 32) <= 8 * kTlSlots, "tmask | pref_t fit in gd at every K of the tile path");
+static_assert((4 + 2) * kTlMaxNodes * (kSpWideLd / 32) + 2 * kTlErow <= 8 * kTlSlots,
+              "tmask | pref_t and desc fit in gd at every K of the tile path");
+static_assert(8 * kTlStage16 <= 4096 && kTlMaxNodes <= 8, "desc: a staged index takes 12 bits, the node 3 above them");
 static_assert(16 * kTlOwn16 >= 8 * kTlAct, "fa fits on stageO");
 static_assert(kTlTail >= kTlAct, "fo and lcnt (one byte per active component) fit where we goes");
-static_assert(8 * (kTlSlots - kTlAct) >= 8 * kTlMaxEdges && 8 * (kTlSlots - kTlAct) >= 8 * kTlAct,
-              "we2 (a float2 per edge) and fu on its way to fa fit in gd behind the gradients of the active components");
+static_assert(kTlTail >= 8 * kTlMaxEdges, "we2 (a float2 per edge) fits where we goes");
+static_assert(8 * (kTlSlots - kTlAct) >= 8 * kTlAct, "fu on its way to fa fits in gd behind the gradients of the active components");
 static_assert(kTlMaxEdges < 256 && kTlEnt <= 256,
               "lcnt: byte counters (a list has at most one entry per edge of its node) and byte cursors (below TE < kTlEnt)");
 static_assert(kTlOffEIo2 + 2 * 32 - kTlOffAmap >= 2 * 16 * kTlMaxEdges, "the pair list of a line-search round fits on amap .. e_io2");
@@ -148,6 +150,19 @@ inline int tl_warps_per_block(int ld) {
     }
     return best;
 }
+
+// Phase profile (tools/phase_clocks.py; only in builds with BIGCLAM_TL_PHASE_CLOCKS, made by tools/build_variant.sh):
+// lane 0 of every warp adds clock64() differences to its own slice of SparseArgs::phase_clocks, kTlPcBuckets x
+// kTlPcSlots counters.  Buckets: 0 hub items, 1 general-path nodes, 1 + nn tiles of nn nodes.  Slots 0-10: the time up
+// to each BIGCLAM_TL_PC(k) of TlWarp::run from the stamp before it (A, B-C1, E-C2, C3-D, G, H, H2, compaction, I, J-K,
+// L), 11: whole items (a tile that falls back included), 12: items.
+constexpr int kTlPcBuckets = 2 + kTlMaxNodes;
+constexpr int kTlPcSlots = 13;
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+#define BIGCLAM_TL_PC(k) pc_mark(k)
+#else
+#define BIGCLAM_TL_PC(k) ((void)0)
+#endif
 
 // ---- mbarrier / bulk-copy primitives (host emulation: the copy happens at once) ----
 #if defined(BIGCLAM_EMU)
@@ -203,12 +218,22 @@ struct TlWarp {
     unsigned long long *mbar;
     unsigned int *tmask;
     int *n_u;
-    unsigned short *slot_c, *plist, *pref_t, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_q;
-    unsigned char *slot_o, *amap, *fo, *lcnt, *ent_e, *ent_a, *erow, *e_ni, *n_want;
+    unsigned short *slot_c, *plist, *pref_t, *desc, *e_soff, *e_cnt, *e_io2, *n_es, *n_sb, *n_ab, *n_m, *n_q;
+    unsigned char *slot_o, *amap, *fo, *lcnt, *ent_e, *ent_a, *erow, *n_want;
     unsigned short *epos;
     signed char *n_js;
     int lane, ld, W;
     unsigned parity;
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+    unsigned long long *pc;          // this warp's counters
+    long long pc_t;
+    int pc_b;
+    __device__ __forceinline__ void pc_mark(int k) {
+        const long long t = clock64();
+        if (lane == 0) pc[pc_b * kTlPcSlots + k] += (unsigned long long)(t - pc_t);
+        pc_t = t;
+    }
+#endif
 
     // the warp region: see the table at kTlOffG
     __device__ __forceinline__ void carve(unsigned char *p, int ld_, int lane_) {
@@ -222,6 +247,7 @@ struct TlWarp {
         ent_val = gd + kTlAct;
         tmask = reinterpret_cast<unsigned int *>(gd);
         pref_t = reinterpret_cast<unsigned short *>(tmask + kTlMaxNodes * W);
+        desc = pref_t + kTlMaxNodes * W;          // flat entry t: its index in stageN (as uint16) | its node << 12
         stageO = p + kTlOffOwn;
         stO = reinterpret_cast<double *>(stageO);
         fa = stO;
@@ -238,7 +264,6 @@ struct TlWarp {
         e_cnt = e_soff + 40;
         e_io2 = reinterpret_cast<unsigned short *>(p + kTlOffEIo2);   // flat entry t of row e: its index is stageN (as uint16) [(e_io2[e] + t) mod 2^16]
         epos = reinterpret_cast<unsigned short *>(p + kTlOffEpos);
-        e_ni = p + kTlOffENi;
         n_u = reinterpret_cast<int *>(p + kTlOffNu);
         n_es = reinterpret_cast<unsigned short *>(p + kTlOffNes);
         n_sb = n_es + 12;
@@ -254,7 +279,7 @@ struct TlWarp {
         fo = p + kTlOffTail;
         lcnt = p + kTlOffTail;
     }
-    // fu of own-entry index o (slot_o, fo): its own-row value, 0 where the node's row has no entry (phases C2-H)
+    // fu of own-entry index o (slot_o, fo): its own-row value, 0 where the node's row has no entry (phases C2 to the compaction)
     __device__ __forceinline__ double fu_of(unsigned o) const { return o != 0xffu ? stO[o] : 0.0; }
     __device__ __forceinline__ double fu_at(int slot) const { return fu_of(slot_o[slot]); }
     // adds 1 to the byte lcnt[i] through the 32-bit word that holds it (no byte carries over: see kTlEnt); returns its old value
@@ -290,6 +315,10 @@ struct TlWarp {
         const bool do_ls = a->do_linesearch != 0;
         const int nsteps = a->nsteps;
         const double max_f = a->max_f;
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+        pc_b = 1 + nn;
+        pc_t = clock64();
+#endif
 
         // ---------------- A. metadata, row headers, staging ----------------
         int ni = 0;
@@ -329,7 +358,6 @@ struct TlWarp {
             e_cnt[lane] = (unsigned short)ce;
             e_io2[lane] = (unsigned short)(8 * soff_e + 4 * (int)sp_vpad((uint32_t)ce) - (incl_c - ce));
             epos[lane] = (unsigned short)(incl_c - ce);
-            e_ni[lane] = (unsigned char)ni;
             if (lane == 0) epos[ne] = (unsigned short)T;
         }
         if (lane < nn) {
@@ -367,6 +395,7 @@ struct TlWarp {
         }
 #endif
         __syncwarp();
+        BIGCLAM_TL_PC(0);
 
         // ---------------- B. own rows: masks of the non-zero components, fu.sumF, fu.fu ----------------
         const int lgs = nn <= 1 ? 5 : nn <= 2 ? 4 : nn <= 4 ? 3 : 2;          // lanes per node: 32 / pow2(nn)
@@ -397,19 +426,25 @@ struct TlWarp {
         unsigned short *ri = sp_idx(rv, (uint32_t)ce);
         if (lane < ne) {
             unsigned char *er = erow + (incl_c - ce);
+            unsigned short *ed = desc + (incl_c - ce);
+            const int d0 = (8 * soff_e + 4 * (int)sp_vpad((uint32_t)ce)) | (ni << 12);
 #pragma unroll 1
-            for (int i = 0; i < ce; ++i) er[i] = (unsigned char)lane;         // flat entry -> row
+            for (int i = 0; i < ce; ++i) {
+                er[i] = (unsigned char)lane;         // flat entry -> row
+                ed[i] = (unsigned short)(d0 + i);    // flat entry -> its index in stageN and its node (C1, C2)
+            }
         }
         __syncwarp();
         unsigned short *stN16 = reinterpret_cast<unsigned short *>(stageN);
         // (from here on the loops over the neighbours' entries are FLAT: entry t of the tile = entry t - epos[row] of row erow[t])
 BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         for (int t = lane; t < T; t += 32) {
-            const int row = erow[t];
-            const int c = stN16[(unsigned short)(e_io2[row] + t)];
-            atomicOr(tmask + (int)e_ni[row] * W + (c >> 5), 1u << (c & 31));
+            const unsigned d = desc[t];
+            const int c = stN16[d & 0xfffu];
+            atomicOr(tmask + (int)(d >> 12) * W + (c >> 5), 1u << (c & 31));
         }
         __syncwarp();
+        BIGCLAM_TL_PC(1);
         // ---------------- E. slots of the touched components (ascending component order per node) ----------------
         int tot_g = 0;
         {
@@ -434,6 +469,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         }
         if (total_slots > kTlSlots) return false;
         if (gv && sub == 0) n_sb[g] = (unsigned short)base_g;
+        if (lane == 0) n_sb[nn] = (unsigned short)total_slots;            // (read again by the compaction, after H2)
 #pragma unroll 1
         for (int i = lane; i < total_slots; i += 32) slot_o[i] = 0xffu;
         __syncwarp();
@@ -450,10 +486,10 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         }
 BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         for (int t = lane; t < T; t += 32) {
-            const int row = erow[t];
-            unsigned short *pc = stN16 + (unsigned short)(e_io2[row] + t);
+            const unsigned d = desc[t];
+            unsigned short *pc = stN16 + (d & 0xfffu);
             const int c = *pc;
-            const int node = e_ni[row];
+            const int node = (int)(d >> 12);
             const int w = c >> 5;
             const unsigned bit = 1u << (c & 31);
             const int slot = (int)n_sb[node] + pref_t[node * W + w] + __popc(tmask[node * W + w] & (bit - 1u));
@@ -461,6 +497,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             *pc = (unsigned short)slot;
         }
         __syncwarp();
+        BIGCLAM_TL_PC(2);
         // ---------------- C3. PRE dots (:162-165), lane = edge ----------------
         double x = 0.0;
         if (lane < ne) {
@@ -500,6 +537,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             }
             llh_g = (S1 - fusf) + fufu;
         }
+        BIGCLAM_TL_PC(3);
         if (!do_ls) {
             if (gv && sub == 0) sp->node_llh[n_u[g]] = llh_g;
             __syncwarp();
@@ -526,6 +564,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             }
             __syncwarp();
         }
+        BIGCLAM_TL_PC(4);
         // ---------------- H. gradient (:168), |g|^2, active components ----------------
         int m_g = 0;
         bool hi_lane = false;
@@ -585,12 +624,13 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             if (gv && sub == 0) n_G2[g] = G2node;
         }
         if (!gv) m_g = 0;
-        int ab_g = 0, maxm = 0;
+        int ab_g = 0, maxm = 0, A = 0;   // A: active components of the tile
 #pragma unroll 1
         for (int q = 0; q < nn; ++q) {
             const int t = __shfl_sync(0xffffffffu, m_g, q << lgs);
             if (q < g) ab_g += t;
             maxm = max(maxm, t);
+            A += t;
         }
         if (gv && sub == 0) { n_ab[g] = (unsigned short)ab_g; n_m[g] = (unsigned short)m_g; }
         // no candidate of any node of the tile can reach MAX_F_ (the largest step is 1): the upper clamp is dropped
@@ -609,27 +649,8 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 En = fma(val, (v.y < 0.0 && v.x > 0.0) ? v.y : 0.0, En);
             }
         }
-        // the active components move to the front, in slot order: fo[a] = own-entry index, gd[a] = grad_c, slot_c[a] = c;
-        // amap (on slot_o): slot -> a
-        int A = 0;
-#pragma unroll 1
-        for (int p0 = 0; p0 < total_slots; p0 += 32) {
-            const int p = p0 + lane;
-            const bool ok = p < total_slots;
-            double2 v = make_double2(0.0, 0.0);
-            int c = 0;
-            if (ok) { v = make_double2(fu_at(p), gd[p]); c = slot_c[p]; }
-            const bool act = ok && (v.x > 0.0 || v.y > 0.0);
-            const unsigned bal = __ballot_sync(0xffffffffu, act);
-            __syncwarp();                        // every lane has read its slot; the writes land at or below them
-            const int an = A + __popc(bal & lt_mask);
-            // (slot_o[p] is read again rather than held across the barrier: amap[p] replaces it only below)
-            if (act && an < kTlAct) { fo[an] = slot_o[p]; gd[an] = v.y; slot_c[an] = (unsigned short)c; }
-            if (ok) amap[p] = act ? (unsigned char)an : (unsigned char)0xffu;   // (an > 254 only in a tile that falls back below)
-            A += __popc(bal);
-            __syncwarp();
-        }
         if (A > kTlAct - 1) return false;                      // (one spare: the padding component, see I)
+        BIGCLAM_TL_PC(5);
         // ---------------- H2. bounds: which (node, candidate) pairs can pass the Armijo test at all ----------------
         // Most candidates can be PROVEN to fail (:181) from what the PRE block already has.  Write the node's objective
         // as phi(nf) = sum_v T(nf.fv) - nf.(sumF - fu), T(x) = S(x) + x, S(x) = log(1 - clamp(exp(-x))) (:166,:179): S is
@@ -655,7 +676,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         // the results are the same bits as those of the exhaustive search (BIGCLAM_F_LS_EXHAUSTIVE, tests/test_gpu_prune.py).
         // Mapping: lane = edge for the per-edge terms, then the lanes of a node's group share its candidates.
         const bool prune = prune_on;
-        float2 *we2 = reinterpret_cast<float2 *>(ent_val);     // (bytes of gd that are free from the compaction to phase I)
+        float2 *we2 = reinterpret_cast<float2 *>(we);          // (we is dead after G)
         if (prune) {
             float lnthr = 3.0e38f, Lp = 0.0f;                  // H_e(s) = 0 up to ln s = lnthr, <= min(cap, ln s + Lp) beyond
             if (vnear > 0.0f) {
@@ -773,7 +794,31 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             if ((svmask >> lane) & 1u) n_sl[__popc(svmask & lt_mask)] = (unsigned char)lane;
         }
         __syncwarp();
+        BIGCLAM_TL_PC(6);
         if (ns > 0) {
+            // the active components move to the front, in slot order: fo[a] = own-entry index, gd[a] = grad_c, slot_c[a] = c;
+            // amap (on slot_o): slot -> a.  (Only phases I-L of a tile with a line-searched node read them: the others
+            // keep their rows, and a node with js < 0 reads none of them in L.)
+            const int total_slots = n_sb[nn];
+            int a0 = 0;
+#pragma unroll 1
+            for (int p0 = 0; p0 < total_slots; p0 += 32) {
+                const int p = p0 + lane;
+                const bool ok = p < total_slots;
+                double2 v = make_double2(0.0, 0.0);
+                int c = 0;
+                if (ok) { v = make_double2(fu_at(p), gd[p]); c = slot_c[p]; }
+                const bool act = ok && (v.x > 0.0 || v.y > 0.0);
+                const unsigned bal = __ballot_sync(0xffffffffu, act);
+                __syncwarp();                        // every lane has read its slot; the writes land at or below them
+                const int an = a0 + __popc(bal & lt_mask);
+                // (slot_o[p] is read again rather than held across the barrier: amap[p] replaces it only below)
+                if (act) { fo[an] = slot_o[p]; gd[an] = v.y; slot_c[an] = (unsigned short)c; }
+                if (ok) amap[p] = act ? (unsigned char)an : (unsigned char)0xffu;
+                a0 += __popc(bal);
+                __syncwarp();
+            }
+            BIGCLAM_TL_PC(7);
             // fa[a] = fu_c onto the own rows' bytes, through ent_val's bytes (free until the fill below).  Padding component A:
             // fu = grad = 0, so every candidate is 0 there and adds exactly nothing — the lockstep loops of the line search
             // read it instead of predicating their bodies
@@ -866,6 +911,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             }
             __syncwarp();
             if (q_lane) n_q[2 * lane + 1] = n_m[lane] > 0 ? lcnt[n_ab[lane] + n_m[lane] - 1] : 0;
+            BIGCLAM_TL_PC(8);
             // ---------------- J. line search (:172-180), two line-searched nodes at a time: lane = (node, trial j) ----------------
             // One loop over the node's active components gives, per candidate: newfu.sfT and newfu.newfu (:176,:180) and,
             // through the components' entry lists, newfu.fv of every edge (xs[edge][trial], component order ascending).
@@ -963,6 +1009,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
             }
         }
         __syncwarp();
+        BIGCLAM_TL_PC(9);
         // ---------------- L. new rows (:183-190) and delta blocks (:191-192) ----------------
         const int js = gv ? (int)n_js[g] : -1;
         const double sstar = s_steps[js >= 0 ? js : 0];
@@ -1067,6 +1114,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                 for (int pr = 0; pr < sp->n_peers; ++pr) sp->peer_hdr[pr][u] = hnew;
         }
         __syncwarp();
+        BIGCLAM_TL_PC(10);
         return true;
     }
 };
@@ -1185,6 +1233,13 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     T.ec = G.ec;
     T.carve(wbase, ld, lane);
     T.mbar = s_mbar + wib;
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+    T.pc = sp.phase_clocks + ((size_t)blockIdx.x * (blockDim.x >> 5) + wib) * (kTlPcBuckets * kTlPcSlots);
+    // one whole item of bucket b, from t0 on
+    auto pc_item = [&](int b, long long t0) {
+        if (lane == 0) { T.pc[b * kTlPcSlots + 11] += (unsigned long long)(clock64() - t0); T.pc[b * kTlPcSlots + 12] += 1ull; }
+    };
+#endif
     if (lane == 0) mbar_init(T.mbar);
     G.clear_dense();
     bool dense_clean = true;      // the two paths share the warp's region: the general path needs its dense vectors zeroed
@@ -1196,7 +1251,13 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
             if (lane == 0) it = atomicAdd(sp.hub_work, 1u);
             it = __shfl_sync(0xffffffffu, it, 0);
             if (it >= (unsigned int)a.n_hub_items) break;
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+            const long long t0 = clock64();
+#endif
             G.template hub_item<kPush>(a.hub_items[it]);
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+            pc_item(0, t0);
+#endif
         }
     }
 
@@ -1208,12 +1269,19 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     while (item < (unsigned int)sp.n_gen || item - (unsigned int)sp.n_gen < (unsigned int)sp.ntiles) {
         unsigned int nxt = 0;
         if (lane == 0) nxt = atomicAdd(a.work_counter, 1u);
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+        const long long t0 = clock64();
+        int pcb = 1;
+#endif
         // nodes for the general path: the item itself, or the nodes of a tile that did not fit (one call site)
         int gen_cnt = 1;
         int64_t gen_pos = (int64_t)a.n_hubs + item;
         const int32_t *gen_col = nullptr;
         if (item >= (unsigned int)sp.n_gen) {
             const TileMeta tm = sp.tiles[item - (unsigned int)sp.n_gen];
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+            pcb = 1 + tm.nn;
+#endif
             dense_clean = false;
             const bool done = T.template run<kPush>(tm);
             if (sp.stats != nullptr && lane == 0) {
@@ -1231,6 +1299,9 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
             G.template node<kPush>(nm.u, nm.deg, gen_col != nullptr ? gen_col : a.col + nm.e0);
             if (gen_col != nullptr) gen_col += nm.deg;
         }
+#ifdef BIGCLAM_TL_PHASE_CLOCKS
+        pc_item(pcb, t0);
+#endif
         item = __shfl_sync(0xffffffffu, nxt, 0);
     }
 }
