@@ -86,7 +86,7 @@ static_assert(2 * kTlOwn16 < 255, "own-entry indices of the slots are bytes (0xf
 
 // The warp region of the tile path.  Buffers whose lifetimes do not overlap share bytes (phases: TlWarp::run):
 //   stageN   neighbour rows  A-I                  | xs (edge x trial)  J-K
-//   gd       tmask | pref_t (48 B per mask word of a node), behind them desc (u16 per entry)  A-C2 | g per slot  G-H2
+//   gd       tmask | pref_t (48 B per mask word of a node), behind them desc (u16 per entry)  A-C2 | sum w fv, then the bound gradient per slot  G-H2
 //            | g of the active components [kTlAct]  compaction-L; behind them fu on its way to fa  I, ent_val  I-J
 //   stageO   own rows  A-I (fu through slot_o, then through fo)   | fa (fu of the active components [kTlAct])  I-L
 //   slot_c   component of a slot  C2-L (below A only after the compaction)  | ent_e, ent_a behind kTlAct  I-J
@@ -153,11 +153,13 @@ inline int tl_warps_per_block(int ld) {
 
 // Phase profile (tools/phase_clocks.py; only in builds with BIGCLAM_TL_PHASE_CLOCKS, made by tools/build_variant.sh):
 // lane 0 of every warp adds clock64() differences to its own slice of SparseArgs::phase_clocks, kTlPcBuckets x
-// kTlPcSlots counters.  Buckets: 0 hub items, 1 general-path nodes, 1 + nn tiles of nn nodes.  Slots 0-10: the time up
-// to each BIGCLAM_TL_PC(k) of TlWarp::run from the stamp before it (A, B-C1, E-C2, C3-D, G, H, H2, compaction, I, J-K,
-// L), 11: whole items (a tile that falls back included), 12: items.
+// kTlPcSlots counters.  Buckets: 0 hub items, 1 general-path nodes, 1 + nn tiles of nn nodes.  Slots 0-15: the time up
+// to each BIGCLAM_TL_PC(k) of TlWarp::run from the stamp before it (A, B-C1, E-C2, C3-D, G, H: gradient loop, H: group
+// reductions and active counts, H: Dp/En walk, H2: lnthr/Lp, H2: per-node fold, H2: candidate walk and bound, H2:
+// svbits/n_sl, compaction, I, J-K, L), kTlPcWhole: whole items (a tile that falls back included), kTlPcItems: items.
 constexpr int kTlPcBuckets = 2 + kTlMaxNodes;
-constexpr int kTlPcSlots = 13;
+constexpr int kTlPcSlots = 18;
+constexpr int kTlPcWhole = kTlPcSlots - 2, kTlPcItems = kTlPcSlots - 1;
 #ifdef BIGCLAM_TL_PHASE_CLOCKS
 #define BIGCLAM_TL_PC(k) pc_mark(k)
 #else
@@ -200,6 +202,12 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned by
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 #endif
+
+// [bounds, H2] the terms of a node's bound that all its candidates share (see H2)
+struct TlBound {
+    double Mp = 0.0, Qn = 0.0, G2p = 0.0, G1 = 0.0, R3 = 0.0, G2node = 0.0;
+    float c0 = 0.0f, c1 = 0.0f, kap0 = 0.0f;
+};
 
 struct TlWarp {
     const StepArgs *a;
@@ -303,6 +311,49 @@ struct TlWarp {
         for (int o = 16; o > 0; o >>= 1)
             if (o < gs) v += __shfl_xor_sync(0xffffffffu, v, o);
         return v;
+    }
+
+    // [bounds, H2] which of the candidates jb + k gs (k < NC) of a node can pass the Armijo test.  Hs[k] = sum_e H_e(s_j)
+    // over the edges r0, r0 + rstep, .. < deg of w2 (lnthr, Lp per edge): 0 up to ln s_j = lnthr, min(cap, ln s_j + Lp)
+    // beyond, viol for Lp < -500.  rstep = 2 (gs = 32): the two half-warps add their partial sums with one shuffle, so
+    // every lane of the warp calls this.  Returns the candidates' bits (those whose bound does not exclude them).
+    template <int NC>
+    __device__ __forceinline__ unsigned cand_bits(const float2 *w2, int r0, int rstep, int deg, int jb, int gs, int jn,
+                                                  float cap_f, bool want, const TlBound &bc) const {
+        float lns[NC], Hs[NC];
+#pragma unroll
+        for (int k = 0; k < NC; ++k) {
+            const int jj = jb + k * gs;
+            lns[k] = (jj < jn) ? s_lns[jj] : -3.0e38f;
+            Hs[k] = 0.0f;
+        }
+#pragma unroll 1
+        for (int r = r0; r < deg; r += rstep) {
+            const float2 tl = w2[r];
+            const bool isv = tl.y < -500.0f;
+            const float vv = -1000.0f - tl.y;
+#pragma unroll
+            for (int k = 0; k < NC; ++k)
+                if (lns[k] > tl.x) Hs[k] += isv ? vv : fminf(cap_f, fmaxf(lns[k] + tl.y, 0.0f));
+        }
+        if (NC == 1 && rstep == 2) Hs[0] += __shfl_xor_sync(0xffffffffu, Hs[0], 16);
+        unsigned bits = 0u;
+        if (want) {
+#pragma unroll
+            for (int k = 0; k < NC; ++k) {
+                const int jj = jb + k * gs;
+                if (jj < jn) {
+                    const double sj = s_steps[jj];
+                    const float sfu = __double2float_ru(sj);
+                    const float kap = fminf(1.0f, __fdividef(bc.kap0, sfu) * 0.9999f);
+                    const double negp = fmin(sj * bc.Qn, bc.R3);
+                    const double bound = negp + fmin(sj * bc.G2p, bc.G1) - sj * ((double)kap * bc.Mp) + (double)(fmaf(Hs[k], 1.00001f, bc.c0) + sfu * bc.c1);
+                    const double rhs = (a->alpha * sj) * bc.G2node;
+                    if (!(bound < rhs * (1.0 - 1.0e-9))) bits |= 1u << jj;
+                }
+            }
+        }
+        return bits;
     }
 
     // One tile.  Returns false (nothing written) when the tile does not fit the warp's buffers.
@@ -586,10 +637,10 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                     const double2 v = make_double2(fu_at(slot), gd[slot]);
                     const double sf = s_sumF[slot_c[slot]];
                     const double gr = (v.y - sf) + v.x;
-                    gd[slot] = gr;
                     G2 = fma(gr, gr, G2);
                     SF2 = fma(sf, sf, SF2);
                     act = (v.x > 0.0 || gr > 0.0);
+                    gd[slot] = act ? gr : 0.0;       // the bound gradient b_c (see the Dp/En walk below)
                     hi_lane |= act && (v.x + gr > max_f);
                     if (act && prune_on) {
                         const float ga = __double2float_ru(fabs(gr)), ff = __double2float_ru(v.x);
@@ -605,16 +656,21 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 }
                 m_g += __popc((__ballot_sync(0xffffffffu, act) >> gsh) & gmask);
             }
+            BIGCLAM_TL_PC(5);
             G2 = group_sum(G2, gs);
             SF2 = group_sum(SF2, gs);
             if (prune_on) {
-                G2n = group_sum(G2n, gs);
-                G2p = group_sum(G2p, gs);
-                r3 = group_sum(r3, gs);
-                g1p = group_sum(g1p, gs);
+                // the five bound-only sums in one butterfly, so that their shuffles are in flight together
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1)
-                    if (o < gs) gmx = fmaxf(gmx, __shfl_xor_sync(0xffffffffu, gmx, o));
+                for (int o = 16; o > 0; o >>= 1) {
+                    if (o < gs) {
+                        G2n += __shfl_xor_sync(0xffffffffu, G2n, o);
+                        G2p += __shfl_xor_sync(0xffffffffu, G2p, o);
+                        r3 += __shfl_xor_sync(0xffffffffu, r3, o);
+                        g1p += __shfl_xor_sync(0xffffffffu, g1p, o);
+                        gmx = fmaxf(gmx, __shfl_xor_sync(0xffffffffu, gmx, o));
+                    }
+                }
                 // sum_act |g_c| (2|g_c| + sumF_c + 3 fu_c) <= 2 |g|^2 + |g| sqrt(2 sum sumF_c^2 + 18 fu.fu) over the touched components
                 const float g2f = __double2float_ru(G2);
                 r4 = fmaf(2.0f, g2f, sqrtf(g2f) * sqrtf(fmaf(2.0f, __double2float_ru(SF2), 18.0f * __double2float_ru(fufu))) * 1.0001f);
@@ -636,21 +692,24 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
         // no candidate of any node of the tile can reach MAX_F_ (the largest step is 1): the upper clamp is dropped
         const bool need_hi = __any_sync(0xffffffffu, hi_lane);
         __syncwarp();
+        BIGCLAM_TL_PC(6);
         // [bounds, see H2] of the edges that are clamped flat: Dp_e = sum_c max(g_c, 0) fv_c and En_e = sum_{c active} min(g_c, 0) fv_c
-        // (a component with g_c < 0 is active iff fu_c > 0)
+        // (a component with g_c < 0 is active iff fu_c > 0).  gd holds the bound gradient b_c = g_c on an active component
+        // and 0 elsewhere, so max(b_c, 0) = max(g_c, 0) (g_c > 0 is active) and min(b_c, 0) = the En term: one dependent
+        // load per entry, the same terms in the same order.  (The compaction's activity test and the values it moves are
+        // those of the active components, unchanged; nothing else reads gd before it.)
         double Dp = 0.0, En = 0.0;
         if (prune_on && (e_low || vnear > 0.0f) && lane < ne) {
 #pragma unroll 1
             for (int i = 0; i < ce; ++i) {
-                const int slot = ri[i];
-                const double2 v = make_double2(fu_at(slot), gd[slot]);
+                const double b = gd[ri[i]];
                 const double val = rv[i];
-                Dp = fma(val, v.y > 0.0 ? v.y : 0.0, Dp);
-                En = fma(val, (v.y < 0.0 && v.x > 0.0) ? v.y : 0.0, En);
+                Dp = fma(val, b > 0.0 ? b : 0.0, Dp);
+                En = fma(val, b < 0.0 ? b : 0.0, En);
             }
         }
         if (A > kTlAct - 1) return false;                      // (one spare: the padding component, see I)
-        BIGCLAM_TL_PC(5);
+        BIGCLAM_TL_PC(7);
         // ---------------- H2. bounds: which (node, candidate) pairs can pass the Armijo test at all ----------------
         // Most candidates can be PROVEN to fail (:181) from what the PRE block already has.  Write the node's objective
         // as phi(nf) = sum_v T(nf.fv) - nf.(sumF - fu), T(x) = S(x) + x, S(x) = log(1 - clamp(exp(-x))) (:166,:179): S is
@@ -707,25 +766,46 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             we2[lane] = make_float2(lnthr, Lp);
             if (!e_low) { Dp = 0.0; En = 0.0; }                // (the node's sums below are over the flat edges only)
         }
+        BIGCLAM_TL_PC(8);
         unsigned svbits = 0u;
         {
             const bool want_g = gv && (n_want[gv ? g : 0] != 0);
             const int jn = nsteps < 16 ? nsteps : 16;
             if (prune) {
-                double sDp = 0.0, sEn = 0.0;
-                float sV = 0.0f;
+                // per-node sums of Dp, En and viol: a node's edges are the consecutive lanes n_es[node] .. n_es[node + 1] - 1,
+                // so a segmented inclusive scan over the edge lanes (ceil(log2 maxdeg) rounds) leaves each node's total on
+                // its last edge lane, and the node's group reads it with one shuffle
+                double sDp = Dp, sEn = En;
+                float sV = violf;
+                {
+                    int e_first = 0;                                            // the first edge lane of this lane's node
 #pragma unroll 1
-                for (int r = 0; r < maxdeg; ++r) {
-                    const int src = (es_g + r) & 31;
-                    const double tD = __shfl_sync(0xffffffffu, Dp, src);
-                    const double tE = __shfl_sync(0xffffffffu, En, src);
-                    const float tV = __shfl_sync(0xffffffffu, violf, src);
-                    if (r < deg_g) { sDp += tD; sEn += tE; sV += tV; }
+                    for (int q = 1; q < nn; ++q) {
+                        const int e = n_es[q];
+                        if (e <= lane) e_first = e;
+                    }
+#pragma unroll 1
+                    for (int o = 1; o < maxdeg; o <<= 1) {
+                        const double tD = __shfl_up_sync(0xffffffffu, sDp, o);
+                        const double tE = __shfl_up_sync(0xffffffffu, sEn, o);
+                        const float tV = __shfl_up_sync(0xffffffffu, sV, o);
+                        if (lane - o >= e_first) { sDp += tD; sEn += tE; sV += tV; }
+                    }
+                    const int last = (es_g + deg_g - 1) & 31;
+                    sDp = __shfl_sync(0xffffffffu, sDp, last);
+                    sEn = __shfl_sync(0xffffffffu, sEn, last);
+                    sV = __shfl_sync(0xffffffffu, sV, last);
+                    if (deg_g == 0) { sDp = 0.0; sEn = 0.0; sV = 0.0; }         // (no edge lane of its own: 'last' is another node's)
                 }
                 __syncwarp();                                                   // (we2 is complete)
+                BIGCLAM_TL_PC(9);
+                const float cap_f = sp->pr_cap;
+                TlBound bc;                      // the node's bound, but for its candidates' edge terms
                 if (want_g) {
-                    const double Mp = (ec.w_lo - 1.0) * sDp, Qn = G2n - (ec.w_lo - 1.0) * sEn;
-                    const float cap_f = sp->pr_cap;
+                    bc.Mp = (ec.w_lo - 1.0) * sDp;
+                    bc.Qn = G2n - (ec.w_lo - 1.0) * sEn;
+                    bc.G2p = G2p;
+                    bc.G2node = G2node;
                     const float fuf = __double2float_ru(fabs(fusf)), fff = __double2float_ru(fufu);
                     const float base = fmaf(2.0f * cap_f, (float)deg_g, __double2float_ru(fabs(llh_g))) + 2.0f * (fuf + fff) + r3;
                     // rounding allowance: twice the worst case of a sum of (4 deg + 3 m + 16) rounded operations on these magnitudes
@@ -734,50 +814,28 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
 #else
                     const float nops = 2.3e-16f * (float)(4 * deg_g + 3 * m_g + 16);
 #endif
-                    const float c0 = fmaf(nops, base, sV) * 1.0001f;
-                    const float c1 = nops * fmaf(2.0f, r4, __double2float_ru(sDp)) * 1.0001f;
+                    bc.c0 = fmaf(nops, base, sV) * 1.0001f;
+                    bc.c1 = nops * fmaf(2.0f, r4, __double2float_ru(sDp)) * 1.0001f;
 #ifdef BIGCLAM_PR_NOG1
-                    const double G1 = 1.0e300;
+                    bc.G1 = 1.0e300;
 #else
-                    const double G1 = (double)(__double2float_ru(max_f) * g1p * 1.0001f);   // >= sum_{g>0} min(s g_c, MAX_F_) g_c
+                    bc.G1 = (double)(__double2float_ru(max_f) * g1p * 1.0001f);   // >= sum_{g>0} min(s g_c, MAX_F_) g_c
 #endif
-                    const double R3 = (double)(r3 * 1.0001f);
+                    bc.R3 = (double)(r3 * 1.0001f);
                     const float fmx = sqrtf(fff) * 1.000001f;                   // >= every fu_c
-                    const float kap0 = (gmx > 0.0f) ? __fdividef(fmaxf(__double2float_rd(max_f) - fmx, 0.0f), gmx) * 0.9999f : 3.0e38f;
-                    // this lane's candidates: sub, sub + gs, sub + 2 gs, sub + 3 gs (gs >= 4); the edge terms of all four in one walk
-                    float lns[4], Hs[4];
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const int jj = sub + k * gs;
-                        lns[k] = (jj < jn) ? s_lns[jj] : -3.0e38f;
-                        Hs[k] = 0.0f;
-                    }
-#pragma unroll 1
-                    for (int r = 0; r < deg_g; ++r) {
-                        const float2 tl = we2[es_g + r];
-                        const bool isv = tl.y < -500.0f;
-                        const float vv = -1000.0f - tl.y;
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            if (lns[k] > tl.x) Hs[k] += isv ? vv : fminf(cap_f, fmaxf(lns[k] + tl.y, 0.0f));
-                    }
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const int jj = sub + k * gs;
-                        if (jj < jn) {
-                            const double sj = s_steps[jj];
-                            const float sfu = __double2float_ru(sj);
-                            const float kap = fminf(1.0f, __fdividef(kap0, sfu) * 0.9999f);
-                            const double negp = fmin(sj * Qn, R3);
-                            const double bound = negp + fmin(sj * G2p, G1) - sj * ((double)kap * Mp) + (double)(fmaf(Hs[k], 1.00001f, c0) + sfu * c1);
-                            const double rhs = (a->alpha * sj) * G2node;
-                            if (!(bound < rhs * (1.0 - 1.0e-9))) svbits |= 1u << jj;
-                        }
-                    }
+                    bc.kap0 = (gmx > 0.0f) ? __fdividef(fmaxf(__double2float_rd(max_f) - fmx, 0.0f), gmx) * 0.9999f : 3.0e38f;
                 }
+                // lane = (candidate, share of the node's edges): 16 / gs candidates per lane at gs <= 16 (sub + k gs); at
+                // gs = 32 one candidate per lane, the two half-groups walking alternate edges
+                const float2 *w2 = we2 + es_g;
+                const int dw = want_g ? deg_g : 0;
+                if (gs >= 16) svbits = cand_bits<1>(w2, gs == 32 ? sub >> 4 : 0, gs >> 4, dw, sub & 15, gs, jn, cap_f, want_g, bc);
+                else if (gs == 8) svbits = cand_bits<2>(w2, 0, 1, dw, sub, gs, jn, cap_f, want_g, bc);
+                else svbits = cand_bits<4>(w2, 0, 1, dw, sub, gs, jn, cap_f, want_g, bc);
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1)
                     if (o < gs) svbits |= __shfl_xor_sync(0xffffffffu, svbits, o);
+                BIGCLAM_TL_PC(10);
             } else if (want_g) {
                 svbits = (1u << jn) - 1u;
             }
@@ -794,7 +852,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             if ((svmask >> lane) & 1u) n_sl[__popc(svmask & lt_mask)] = (unsigned char)lane;
         }
         __syncwarp();
-        BIGCLAM_TL_PC(6);
+        BIGCLAM_TL_PC(11);
         if (ns > 0) {
             // the active components move to the front, in slot order: fo[a] = own-entry index, gd[a] = grad_c, slot_c[a] = c;
             // amap (on slot_o): slot -> a.  (Only phases I-L of a tile with a line-searched node read them: the others
@@ -818,7 +876,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
                 a0 += __popc(bal);
                 __syncwarp();
             }
-            BIGCLAM_TL_PC(7);
+            BIGCLAM_TL_PC(12);
             // fa[a] = fu_c onto the own rows' bytes, through ent_val's bytes (free until the fill below).  Padding component A:
             // fu = grad = 0, so every candidate is 0 there and adds exactly nothing — the lockstep loops of the line search
             // read it instead of predicating their bodies
@@ -911,7 +969,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UF)
             }
             __syncwarp();
             if (q_lane) n_q[2 * lane + 1] = n_m[lane] > 0 ? lcnt[n_ab[lane] + n_m[lane] - 1] : 0;
-            BIGCLAM_TL_PC(8);
+            BIGCLAM_TL_PC(13);
             // ---------------- J. line search (:172-180), two line-searched nodes at a time: lane = (node, trial j) ----------------
             // One loop over the node's active components gives, per candidate: newfu.sfT and newfu.newfu (:176,:180) and,
             // through the components' entry lists, newfu.fv of every edge (xs[edge][trial], component order ascending).
@@ -1009,7 +1067,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
             }
         }
         __syncwarp();
-        BIGCLAM_TL_PC(9);
+        BIGCLAM_TL_PC(14);
         // ---------------- L. new rows (:183-190) and delta blocks (:191-192) ----------------
         const int js = gv ? (int)n_js[g] : -1;
         const double sstar = s_steps[js >= 0 ? js : 0];
@@ -1114,7 +1172,7 @@ BIGCLAM_UNROLL(BIGCLAM_TL_UJ)
                 for (int pr = 0; pr < sp->n_peers; ++pr) sp->peer_hdr[pr][u] = hnew;
         }
         __syncwarp();
-        BIGCLAM_TL_PC(10);
+        BIGCLAM_TL_PC(15);
         return true;
     }
 };
@@ -1237,7 +1295,7 @@ __global__ void __launch_bounds__(kTlThreads, kTlBlocksPerSM) tile_step_kernel(c
     T.pc = sp.phase_clocks + ((size_t)blockIdx.x * (blockDim.x >> 5) + wib) * (kTlPcBuckets * kTlPcSlots);
     // one whole item of bucket b, from t0 on
     auto pc_item = [&](int b, long long t0) {
-        if (lane == 0) { T.pc[b * kTlPcSlots + 11] += (unsigned long long)(clock64() - t0); T.pc[b * kTlPcSlots + 12] += 1ull; }
+        if (lane == 0) { T.pc[b * kTlPcSlots + kTlPcWhole] += (unsigned long long)(clock64() - t0); T.pc[b * kTlPcSlots + kTlPcItems] += 1ull; }
     };
 #endif
     if (lane == 0) mbar_init(T.mbar);
